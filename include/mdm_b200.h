@@ -130,6 +130,9 @@ typedef struct mdm_net_cfg {
   int32_t has_cond_emb;
   int32_t masked_cross_attention;
   int32_t num_heads; /* 8 (unet.py:245) */
+  /* UNetConfig.num_lm_head_layers of the innermost level: SelfAttention1DBlock layers over the conditioning tokens
+   * after lm_proj (unet.py:766-771,849-853); needs has_cond_emb */
+  int32_t num_lm_head_layers;
 } mdm_net_cfg;
 
 typedef struct mdm_net mdm_net;
@@ -324,6 +327,18 @@ int mdm_op_attention_fwd(const void* qkv16, const void* kv16, const float* mask,
 int mdm_op_attention_bwd(const void* qkv16, const void* kv16, const float* mask, const void* dO16, const void* h16,
                          const void* oself16, const float* stats, int B, int T, int S, int C, int heads, float* Dterm,
                          float* dq32, void* dqkv16, void* dkv16, mdm_stream_t stream);
+
+/* ---------------------------------------------------------------- token self-attention (single operator, for tests)
+ * SelfAttention1D.attention of the lm_head layers (models/unet.py:350-375): qkv16 (B*T, 3D) fp16 = [q|k|v] thirds,
+ * `heads` heads of d = D/heads columns (d a multiple of 8, 8 <= d <= 256), key mask (B,T) fp32 0/1 or NULL.
+ * o16 (B*T, D) = softmax(qk^T/sqrt d, masked keys -inf) v; stats (B,heads,T,2) fp32 is the residue for the backward
+ * (may be NULL for inference). A sample whose keys are all masked gets zero output rows and zero gradients. */
+int mdm_op_token_attention_fwd(const void* qkv16, const float* mask, int B, int T, int D, int heads, void* o16,
+                               float* stats, mdm_stream_t stream);
+/* Backward: dO16 (B*T, D) -> dqkv16 (B*T, 3D). Dterm (B,heads,T) and dq32 (B*T, D) are fp32 scratch. */
+int mdm_op_token_attention_bwd(const void* qkv16, const float* mask, const void* dO16, const void* o16,
+                               const float* stats, int B, int T, int D, int heads, float* Dterm, float* dq32,
+                               void* dqkv16, mdm_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -14,19 +14,20 @@
 
 #include <type_traits>
 
+#include "attn_common.cuh"
 #include "engine.cuh"
 #include "mdm_b200.h"
 #include "ptx.cuh"
 
 namespace mdm {
 using namespace ptx;
+using namespace attn;
 
 namespace {
 
 constexpr int AT_THREADS = 256;   // forward: two warpgroups, 64 queries each
 constexpr int BWD_THREADS = 256;  // backward: two warpgroups, 64 keys each
 constexpr int TILE = 128;           // queries per CTA (fwd) / keys per CTA (bwd); key chunk size
-constexpr int KB_BYTES = 128 * 128; // one [128 rows][64 fp16] k-block / slab
 
 struct AttnParams {
   int T, S, d, heads, B;
@@ -45,36 +46,6 @@ struct AttnParams {
   __half* dqkv16;      // [B*T][3C]: dK at +C, dV at +2C
   __half* dkv16;       // [B*S][2C]: dKc at +0, dVc at +C
 };
-
-__device__ __forceinline__ uint64_t desc_k(uint32_t base, int k16) {  // K-major, 16-element step k16
-  return make_smem_desc_sw128(base + k16 * 32, 16, 1024);
-}
-__device__ __forceinline__ uint64_t desc_mn(uint32_t base, int k16, uint32_t slab_bytes) {  // MN-major
-  return make_smem_desc_sw128(base + k16 * 2048, slab_bytes, 1024);
-}
-
-// Accumulator fragment of a 64 x N wgmma in one thread: element e = 4 j + 2 h + u holds row
-// (warp % 4) * 16 + lane / 4 + 8 h and column 8 j + 2 (lane % 4) + u of the warpgroup's 64-row block.
-__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
-  __half2 h = __floats2half2_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-// the 16-column k step t of a 64 x N accumulator as the A operand (four fp16x2 registers) of the next wgmma
-__device__ __forceinline__ void frag_a(const float* v, int t, uint32_t* a) {
-  a[0] = pack_half2(v[8 * t + 0], v[8 * t + 1]);
-  a[1] = pack_half2(v[8 * t + 2], v[8 * t + 3]);
-  a[2] = pack_half2(v[8 * t + 4], v[8 * t + 5]);
-  a[3] = pack_half2(v[8 * t + 6], v[8 * t + 7]);
-}
-// row reductions over the four threads (lane % 4) that share an accumulator row
-__device__ __forceinline__ float quad_max(float x) {
-  x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 1));
-  return fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 2));
-}
-__device__ __forceinline__ float quad_sum(float x) {
-  x += __shfl_xor_sync(0xffffffffu, x, 1);
-  return x + __shfl_xor_sync(0xffffffffu, x, 2);
-}
 
 // ------------------------------------------------------------------------------------------ forward
 // Two warpgroups, 64 query rows each. S (64 x 128 keys) and O (64 x DN) live in registers; P goes from the S
@@ -564,21 +535,6 @@ EncodeTiledFn encode_fn() {
   }
   return fn;
 }
-// 4-D fp16 view (inner d, rows, slots, batch), box {64, 128, 1, 1}
-void head_map(CUtensorMap* m, const void* ptr, int d, int rows, long long row_stride, int slots, long long slot_stride,
-              int batch, long long batch_stride) {
-  EncodeTiledFn fn = encode_fn();
-  MDM_CHECK(fn != nullptr, "cuTensorMapEncodeTiled unavailable");
-  cuuint64_t dims[4] = {static_cast<cuuint64_t>(d), static_cast<cuuint64_t>(rows), static_cast<cuuint64_t>(slots),
-                        static_cast<cuuint64_t>(batch)};
-  cuuint64_t str[3] = {static_cast<cuuint64_t>(row_stride) * 2, static_cast<cuuint64_t>(slot_stride) * 2,
-                       static_cast<cuuint64_t>(batch_stride) * 2};
-  cuuint32_t box[4] = {64, 128, 1, 1}, es[4] = {1, 1, 1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr), dims, str, box, es,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  MDM_CHECK(r == CUDA_SUCCESS, "attention tensor map encode failed");
-}
 
 // Calls f(std::integral_constant<int, DN>) with DN = the head dimension rounded up to 16 (the wgmma N of the
 // products with d columns).
@@ -597,6 +553,26 @@ void with_head_width(int d, F&& f) {
 }
 
 }  // namespace
+
+void attn::head_map(CUtensorMap* m, const void* ptr, int d, int rows, long long row_stride, int slots,
+                    long long slot_stride, int batch, long long batch_stride, int box_rows) {
+  EncodeTiledFn fn = encode_fn();
+  MDM_CHECK(fn != nullptr, "cuTensorMapEncodeTiled unavailable");
+  cuuint64_t dims[4] = {static_cast<cuuint64_t>(d), static_cast<cuuint64_t>(rows), static_cast<cuuint64_t>(slots),
+                        static_cast<cuuint64_t>(batch)};
+  cuuint64_t str[3] = {static_cast<cuuint64_t>(row_stride) * 2, static_cast<cuuint64_t>(slot_stride) * 2,
+                       static_cast<cuuint64_t>(batch_stride) * 2};
+  cuuint32_t box[4] = {64, static_cast<cuuint32_t>(box_rows), 1, 1}, es[4] = {1, 1, 1, 1};
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr), dims, str, box, es,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  MDM_CHECK(r == CUDA_SUCCESS, "attention tensor map encode failed");
+}
+
+void attn::cast_rows_f16(const float* in, __half* out, long long rows, int C, int ld_out, cudaStream_t st) {
+  cast_strided_kernel<<<132 * 8, 256, 0, st>>>(in, out, rows, C, ld_out);
+  ++g_launch_count;
+}
 
 // ------------------------------------------------------------------------------------------ host API
 void attention_forward(const __half* qkv, const __half* kv, const float* mask, int B, int T, int S, int C, int heads,
@@ -669,8 +645,7 @@ void attention_backward(const __half* qkv, const __half* kv, const float* mask, 
   ++g_launch_count;
   MDM_CUDA(cudaGetLastError());
   // dQ: fp32 accumulator -> fp16 into the q third of dqkv
-  cast_strided_kernel<<<132 * 8, 256, 0, st>>>(dq32, dqkv16, rows, C, 3 * C);
-  ++g_launch_count;
+  cast_rows_f16(dq32, dqkv16, rows, C, 3 * C, st);
 }
 
 }  // namespace mdm

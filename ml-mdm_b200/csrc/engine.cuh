@@ -192,4 +192,12 @@ void attention_backward(const __half* qkv, const __half* kv, const float* mask, 
                         const __half* oself16, const float* stats, int B, int T, int S, int C, int heads, float* Dterm,
                         float* dq32, __half* dqkv16, __half* dkv16, cudaStream_t st);
 
+// Masked self-attention over text tokens (token_attention.cu): qkv [B*T][3D], mask [B][T] or null -> o16 [B*T][D];
+// stats [B][heads][T][2] (may be null without a backward). Backward: Dterm [B][heads][T] and dq32 [B*T][D] scratch.
+void token_attention_forward(const __half* qkv, const float* mask, int B, int T, int D, int heads, __half* o16,
+                             float* stats, cudaStream_t st);
+void token_attention_backward(const __half* qkv, const float* mask, const __half* dO, const __half* o16,
+                              const float* stats, int B, int T, int D, int heads, float* Dterm, float* dq32,
+                              __half* dqkv16, cudaStream_t st);
+
 }  // namespace mdm

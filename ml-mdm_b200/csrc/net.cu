@@ -328,6 +328,26 @@ struct Net {
         add_param(pre + "lm_proj.weight", {cfg.cond_dim, cfg.lm_dim}, 1);
         add_param(pre + "lm_proj.bias", {cfg.cond_dim}, 0);
       }
+      if (L.innermost) {
+        MDM_CHECK(cfg.num_lm_head_layers >= 0 && (cfg.num_lm_head_layers == 0 || cfg.has_cond_emb),
+                  "lm_head layers exist only beside cond_emb");
+        const int D = cfg.cond_dim;
+        for (int i = 0; i < cfg.num_lm_head_layers; ++i) {  // SelfAttention1DBlock (unet.py:439-446)
+          const std::string h = pre + "lm_head." + std::to_string(i);
+          add_param(h + ".attn.norm.weight", {D}, 0);
+          add_param(h + ".attn.norm.bias", {D}, 0);
+          add_param(h + ".attn.qkv.weight", {3 * D, D}, 1);
+          add_param(h + ".attn.qkv.bias", {3 * D}, 0);
+          add_param(h + ".attn.proj_out.weight", {D, D}, 1);
+          add_param(h + ".attn.proj_out.bias", {D}, 0);
+          add_param(h + ".mlp.main.0.weight", {D}, 0);
+          add_param(h + ".mlp.main.0.bias", {D}, 0);
+          add_param(h + ".mlp.main.1.weight", {4 * D, D}, 1);
+          add_param(h + ".mlp.main.1.bias", {4 * D}, 0);
+          add_param(h + ".mlp.main.3.weight", {D, 4 * D}, 1);
+          add_param(h + ".mlp.main.3.bias", {D}, 0);
+        }
+      }
       levels.push_back(L);
       pre += "inner_unet.";
     }
@@ -1239,7 +1259,8 @@ struct Net {
     cs.S = S;
     cs.cd = cfg.cond_dim;
     cs.lm = io->lm;
-    cs.mask = io->lm_mask;
+    // with lm_head layers and unmasked cross-attention the pooled y is the plain mean over all tokens (unet.py:854-856)
+    cs.mask = (cfg.num_lm_head_layers > 0 && !cfg.masked_cross_attention) ? nullptr : io->lm_mask;
     cs.cross_mask = cfg.masked_cross_attention ? io->lm_mask : nullptr;
     if (cfg.cond_dim <= 0) return;
     const long long crow = static_cast<long long>(B) * S;
@@ -1257,10 +1278,25 @@ struct Net {
       e.bias = b.w;
       e.out_f32 = cs.cond32;
       E.gemm_nt(cs.lm16, cfg.lm_dim, w.w16, cfg.lm_dim, static_cast<int>(crow), cfg.cond_dim, cfg.lm_dim, e);
+      if (E.training) {
+        // runs after the lm_head backward closures have turned cs.dcond into the gradient of lm_proj's output
+        E.tape.push_back([=]() {
+          if (cs.dcond == nullptr) return;
+          Engine& E = eng;
+          const LevelSpec& L = levels.back();
+          Param &w = P(L.pre + "lm_proj.weight"), &b = P(L.pre + "lm_proj.bias");
+          __half* d16 = E.alloc<__half>(crow * cfg.cond_dim);
+          cast_colsum(cs.dcond, d16, crow, cfg.cond_dim, b.g, inv_scale(), E.st);
+          linear_bwd(d16, cfg.cond_dim, static_cast<int>(crow), cfg.cond_dim, cfg.lm_dim, cs.lm16, cfg.lm_dim, w,
+                     nullptr, false, nullptr, 0);
+          E.rel(d16);
+        });
+      }
     } else {
       MDM_CHECK(!io->apply_lm_mask, "apply_lm_mask is only built for models with an lm_proj layer");
       cs.cond32 = const_cast<float*>(io->lm);
     }
+    for (int i = 0; i < cfg.num_lm_head_layers; ++i) lm_head_fwd(L.pre + "lm_head." + std::to_string(i), B, S);
     {  // LayerNorm(cond) without its affine part, once per forward (31 blocks share it; unet.py:263,304)
       cs.xhat16 = E.alloc<__half>(crow * cfg.cond_dim);
       cs.lnstats = E.alloc<float>(crow * 2);
@@ -1287,7 +1323,7 @@ struct Net {
         cast_colsum(cs.dcemb, d16, B, td, nullptr, nullptr, E.st);
         float* dy = E.alloc<float>(static_cast<long long>(B) * cfg.cond_dim);
         linear_bwd(d16, td, B, td, cfg.cond_dim, cs.y16, cfg.cond_dim, cw, nullptr, false, dy, 0);
-        if (cfg.has_lm_proj) {
+        if (cfg.has_lm_proj || cfg.num_lm_head_layers > 0) {
           if (cs.dcond == nullptr) cs.dcond = E.alloc<float>(crow * cfg.cond_dim);
           masked_mean_bwd(dy, cs.mask, cs.dcond, cs.dcond_init ? 1 : 0, B, S, cfg.cond_dim, E.st);
           cs.dcond_init = true;
@@ -1301,14 +1337,123 @@ struct Net {
                       crow, cfg.cond_dim, E.st);
         cs.dcond_init = true;
       }
-      if (cfg.has_lm_proj && cs.dcond != nullptr) {
-        Param &w = P(L.pre + "lm_proj.weight"), &b = P(L.pre + "lm_proj.bias");
-        __half* d16 = E.alloc<__half>(crow * cfg.cond_dim);
-        cast_colsum(cs.dcond, d16, crow, cfg.cond_dim, b.g, inv_scale(), E.st);
-        linear_bwd(d16, cfg.cond_dim, static_cast<int>(crow), cfg.cond_dim, cfg.lm_dim, cs.lm16, cfg.lm_dim, w, nullptr,
-                   false, nullptr, 0);
-        E.rel(d16);
+    });
+  }
+
+  // One SelfAttention1DBlock of lm_head (unet.py:316-446) on the fp32 token stream cs.cond32 (B*S rows of D):
+  //   x1 = x + proj_out(attn(qkv(LayerNorm(x)), mask)),  x2 = x1 + W3 gelu(W1 LayerNorm(x1) + b1) + b3
+  // cs.cond32 becomes x2. The backward closure turns cs.dcond (gradient of x2) into the gradient of x, in place.
+  void lm_head_fwd(const std::string& pre, int B, int S) {
+    Engine& E = eng;
+    const int D = cfg.cond_dim, nh = cfg.num_heads;
+    const long long rows = static_cast<long long>(B) * S;
+    const int irows = static_cast<int>(rows);
+    const float* mask = cs.cross_mask;  // the reference passes cond_mask only with masked_cross_attention
+    Param &nw = P(pre + ".attn.norm.weight"), &nb = P(pre + ".attn.norm.bias");
+    Param &qw = P(pre + ".attn.qkv.weight"), &qb = P(pre + ".attn.qkv.bias");
+    Param &pw = P(pre + ".attn.proj_out.weight"), &pb = P(pre + ".attn.proj_out.bias");
+    Param &mw0 = P(pre + ".mlp.main.0.weight"), &mb0 = P(pre + ".mlp.main.0.bias");
+    Param &mw1 = P(pre + ".mlp.main.1.weight"), &mb1 = P(pre + ".mlp.main.1.bias");
+    Param &mw3 = P(pre + ".mlp.main.3.weight"), &mb3 = P(pre + ".mlp.main.3.bias");
+    const float* x = cs.cond32;
+    float* ln1 = E.alloc<float>(rows * 2);
+    __half* xn16 = E.alloc<__half>(rows * D);
+    layernorm_fwd(x, nw.w, nb.w, xn16, ln1, rows, D, E.st);
+    __half* qkv = E.alloc<__half>(rows * 3 * D);
+    {
+      Epi e;
+      e.bias = qb.w;
+      e.out_f16 = qkv;
+      E.gemm_nt(xn16, D, qw.w16, D, irows, 3 * D, D, e);
+    }
+    __half* o16 = E.alloc<__half>(rows * D);
+    float* stats = E.training ? E.alloc<float>(rows * nh * 2) : nullptr;
+    token_attention_forward(qkv, mask, B, S, D, nh, o16, stats, E.st);
+    float* x1 = E.alloc<float>(rows * D);
+    {
+      Epi e;
+      e.bias = pb.w;
+      e.residual = x;
+      e.out_f32 = x1;
+      E.gemm_nt(o16, D, pw.w16, D, irows, D, D, e);
+    }
+    float* ln2 = E.alloc<float>(rows * 2);
+    __half* y16 = E.alloc<__half>(rows * D);
+    layernorm_fwd(x1, mw0.w, mb0.w, y16, ln2, rows, D, E.st);
+    __half* u16 = E.training ? E.alloc<__half>(rows * 4 * D) : nullptr;  // pre-activation: only the backward needs it
+    __half* g16 = E.alloc<__half>(rows * 4 * D);
+    {
+      Epi e;
+      e.bias = mb1.w;
+      e.out_f16 = u16;
+      e.out_act_f16 = g16;
+      e.act = ACT_GELU;
+      E.gemm_nt(y16, D, mw1.w16, D, irows, 4 * D, D, e);
+    }
+    float* x2 = E.alloc<float>(rows * D);
+    {
+      Epi e;
+      e.bias = mb3.w;
+      e.residual = x1;
+      e.out_f32 = x2;
+      E.gemm_nt(g16, 4 * D, mw3.w16, 4 * D, irows, D, 4 * D, e);
+    }
+    cs.cond32 = x2;
+    if (!E.training) {
+      E.rel(ln1); E.rel(xn16); E.rel(qkv); E.rel(o16);
+      E.rel(x1); E.rel(ln2); E.rel(y16); E.rel(g16);
+      return;
+    }
+    E.tape.push_back([=]() {
+      if (cs.dcond == nullptr) return;  // no gradient reached the tokens
+      Engine& E = eng;
+      Param &nw = P(pre + ".attn.norm.weight"), &nb = P(pre + ".attn.norm.bias");
+      Param &qw = P(pre + ".attn.qkv.weight"), &qb = P(pre + ".attn.qkv.bias");
+      Param &pw = P(pre + ".attn.proj_out.weight"), &pb = P(pre + ".attn.proj_out.bias");
+      Param &mw0 = P(pre + ".mlp.main.0.weight"), &mb0 = P(pre + ".mlp.main.0.bias");
+      Param &mw1 = P(pre + ".mlp.main.1.weight"), &mb1 = P(pre + ".mlp.main.1.bias");
+      Param &mw3 = P(pre + ".mlp.main.3.weight"), &mb3 = P(pre + ".mlp.main.3.bias");
+      float* g = cs.dcond;
+      // MLP: dW3, then dU = (dX2 W3) * gelu'(U) straight out of the dgrad epilogue
+      __half* d16 = E.alloc<__half>(rows * D);
+      cast_colsum(g, d16, rows, D, mb3.g, inv_scale(), E.st);
+      linear_bwd(d16, D, irows, D, 4 * D, g16, 4 * D, mw3, nullptr, false, nullptr, 0);
+      __half* du16 = E.alloc<__half>(rows * 4 * D);
+      {
+        Epi e;
+        e.out_f16 = du16;
+        e.gelu_grad_src = u16;
+        E.gemm_nn(d16, D, mw3.w16, 4 * D, irows, 4 * D, D, e);
       }
+      E.rel(d16);
+      float* dy32 = E.alloc<float>(rows * D);
+      linear_bwd(du16, 4 * D, irows, 4 * D, D, y16, D, mw1, &mb1, true, dy32, 0);
+      E.rel(du16);
+      layernorm_bwd(x1, mw0.w, ln2, dy32, g, 1, mw0.g, mb0.g, inv_scale(), rows, D, E.st);  // g: gradient of x1
+      E.rel(dy32);
+      // attention: dW_proj, dO = dX1 W_proj, token attention backward, then qkv and its LayerNorm
+      __half* dx16 = E.alloc<__half>(rows * D);
+      cast_colsum(g, dx16, rows, D, pb.g, inv_scale(), E.st);
+      linear_bwd(dx16, D, irows, D, D, o16, D, pw, nullptr, false, nullptr, 0);
+      __half* do16 = E.alloc<__half>(rows * D);
+      {
+        Epi e;
+        e.out_f16 = do16;
+        E.gemm_nn(dx16, D, pw.w16, D, irows, D, D, e);
+      }
+      E.rel(dx16);
+      __half* dqkv = E.alloc<__half>(rows * 3 * D);
+      float* Dterm = E.alloc<float>(rows * nh);
+      float* dq32 = E.alloc<float>(rows * D);
+      token_attention_backward(qkv, mask, do16, o16, stats, B, S, D, nh, Dterm, dq32, dqkv, E.st);
+      E.rel(Dterm);
+      E.rel(dq32);
+      E.rel(do16);
+      float* dn32 = E.alloc<float>(rows * D);
+      linear_bwd(dqkv, 3 * D, irows, 3 * D, D, xn16, D, qw, &qb, true, dn32, 0);
+      E.rel(dqkv);
+      layernorm_bwd(x, nw.w, ln1, dn32, g, 1, nw.g, nb.g, inv_scale(), rows, D, E.st);  // g: gradient of x
+      E.rel(dn32);
     });
   }
 

@@ -40,6 +40,7 @@ class NetCfg(C.Structure):
         ("has_cond_emb", C.c_int32),
         ("masked_cross_attention", C.c_int32),
         ("num_heads", C.c_int32),
+        ("num_lm_head_layers", C.c_int32),
     ]
 
 
@@ -113,6 +114,7 @@ def build_net_cfg(module) -> NetCfg:
     nc.has_cond_emb = int(inner.cond_emb is not None)
     nc.masked_cross_attention = int(icfg.masked_cross_attention)
     nc.num_heads = 8
+    nc.num_lm_head_layers = len(inner.lm_head) if getattr(inner, "lm_head", None) is not None else 0
     return nc
 
 

@@ -76,6 +76,39 @@ class _Attention(nn.Module):
             )
 
 
+class _MLP(nn.Module):
+    """Parameters of the reference MLP (unet.py:425-436): x + Linear(GELU(Linear(LayerNorm(x))))."""
+
+    def __init__(self, channels, multiplier=4):
+        super().__init__()
+        self.main = nn.Sequential(
+            nn.LayerNorm(channels),
+            nn.Linear(channels, multiplier * channels),
+            nn.GELU(),
+            zero_module(nn.Linear(multiplier * channels, channels)),
+        )
+
+
+class _SelfAttention1D(nn.Module):
+    """Parameters of the reference SelfAttention1D without FFN (unet.py:316-346)."""
+
+    def __init__(self, channels):
+        super().__init__()
+        self.norm = nn.LayerNorm(channels)
+        self.qkv = nn.Linear(channels, channels * 3)
+        self.proj_out = zero_module(nn.Linear(channels, channels))
+
+
+class SelfAttention1DBlock(nn.Module):
+    """Parameters of one lm_head layer (reference SelfAttention1DBlock, unet.py:439-446): 8-head self-attention over
+    the conditioning tokens, then an MLP."""
+
+    def __init__(self, channels):
+        super().__init__()
+        self.attn = _SelfAttention1D(channels)
+        self.mlp = _MLP(channels)
+
+
 class _Block(nn.Module):
     """Parameters of one resolution block (reference ResNetBlock, unet.py:449-532)."""
 
@@ -105,9 +138,9 @@ class UNet(nn.Module):
         nres = _ints(config.num_resnets_per_resolution, L)
         nattn = _ints(config.num_attention_layers, L)
         attn_levels = _ints(config.attention_levels)
-        if _cfg_get(config, "temporal_mode", False) or _cfg_get(config, "num_lm_head_layers", 0):
-            raise NotImplementedError("temporal mode / lm_head layers are inactive in all shipped configs "
-                                      "and are not part of the native path (SURVEY.md 8f)")
+        if _cfg_get(config, "temporal_mode", False):
+            raise NotImplementedError("temporal mode is inactive in all shipped configs "
+                                      "and is not part of the native path (SURVEY.md 8f)")
         # mirrors unet.py:588-598: projected conditioning replaces the feature dim
         self.input_conditioning_feature_dim = config.conditioning_feature_dim
         if config.conditioning_feature_dim > 0 and config.conditioning_feature_proj_dim > 0:
@@ -169,7 +202,8 @@ class UNet(nn.Module):
         if has_cond_emb:
             if config.conditioning_feature_proj_dim > 0:
                 self.lm_proj = nn.Linear(self.input_conditioning_feature_dim, cond_dim)
-            self.lm_head = nn.ModuleList([])
+            self.lm_head = nn.ModuleList(
+                [SelfAttention1DBlock(cond_dim) for _ in range(_cfg_get(config, "num_lm_head_layers", 0) or 0)])
         self.is_temporal = []
         self._native = None
 
