@@ -94,6 +94,11 @@ int mdm_profile_dump(const char* path);
 
 int mdm_gemm_raw(const mdm_tmap_spec* A, const mdm_tmap_spec* B, int a_mn, int b_mn,
                  const mdm_gemm_params* p, mdm_stream_t stream);
+/* mdm_gemm_raw with the split operand planes the engine gives its weight products: b_lo (or NULL) is a second fp16
+ * plane laid out exactly like B, a_lo (or NULL) one laid out exactly like A; the result is A B + A b_lo + a_lo B.
+ * MDM_GEMM_CONV_WGRAD uses neither plane, and a_lo is used only with a K-major A (a_mn = 0). */
+int mdm_gemm_raw_split(const mdm_tmap_spec* A, const mdm_tmap_spec* B, int a_mn, int b_mn, const mdm_gemm_params* p,
+                       const void* b_lo, const void* a_lo, mdm_stream_t stream);
 
 
 /* ---------------------------------------------------------------- the (nested) U-Net denoiser */

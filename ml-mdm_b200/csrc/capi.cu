@@ -83,14 +83,19 @@ long long mdm_abi_sizeof(int which) {
   }
 }
 
-int mdm_gemm_raw(const mdm_tmap_spec* A, const mdm_tmap_spec* B, int a_mn, int b_mn,
-                 const mdm_gemm_params* p, mdm_stream_t stream) {
-  int rc = mdm::launch_gemm(*A, *B, a_mn, b_mn, *p, static_cast<cudaStream_t>(stream));
+int mdm_gemm_raw_split(const mdm_tmap_spec* A, const mdm_tmap_spec* B, int a_mn, int b_mn, const mdm_gemm_params* p,
+                       const void* b_lo, const void* a_lo, mdm_stream_t stream) {
+  int rc = mdm::launch_gemm(*A, *B, a_mn, b_mn, *p, static_cast<cudaStream_t>(stream), b_lo, a_lo);
   if (rc != 0) {
     mdm::set_error("mdm_gemm_raw: launch failed (%d: %s)", rc,
                    rc > 0 ? cudaGetErrorString(static_cast<cudaError_t>(rc)) : "invalid arguments");
     return rc > 0 ? -rc : rc;
   }
   return 0;
+}
+
+int mdm_gemm_raw(const mdm_tmap_spec* A, const mdm_tmap_spec* B, int a_mn, int b_mn,
+                 const mdm_gemm_params* p, mdm_stream_t stream) {
+  return mdm_gemm_raw_split(A, B, a_mn, b_mn, p, nullptr, nullptr, stream);
 }
 }

@@ -124,3 +124,12 @@ def gemm_raw(A, B, a_mn, b_mn, params, stream=0):
                            C.c_void_p(stream)),
         "mdm_gemm_raw",
     )
+
+
+def gemm_raw_split(A, B, a_mn, b_mn, params, b_lo=0, a_lo=0, stream=0):
+    """gemm_raw with second fp16 planes of B and of a K-major A (device pointers, 0 = none): A B + A b_lo + a_lo B."""
+    check(
+        lib().mdm_gemm_raw_split(C.byref(A), C.byref(B), int(a_mn), int(b_mn), C.byref(params),
+                                 C.c_void_p(b_lo or None), C.c_void_p(a_lo or None), C.c_void_p(stream)),
+        "mdm_gemm_raw_split",
+    )
