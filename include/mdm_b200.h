@@ -123,6 +123,9 @@ typedef struct mdm_level_cfg {
   int32_t skip_normalization; /* NestedUNetConfig.skip_normalization (outer levels only) */
   int32_t has_micro_scale;    /* micro_conditioning == "scale:<default>" */
   float micro_scale_default;
+  /* ResNetConfig.dropout in [0, 1]: nn.Dropout between SiLU(norm2) and conv2 of every ResNet of this level
+   * (unet.py:208,233-235), applied when mdm_net_io.dropout is 1 */
+  float dropout;
 } mdm_level_cfg;
 
 typedef struct mdm_net_cfg {
@@ -175,10 +178,18 @@ typedef struct mdm_net_io {
   /* 1: lm is the raw encoder output and is multiplied by lm_mask on the way in (what language_models/factory.py:101
    * does as a separate (B,S,D) pass before the model is called); needs lm_mask and the lm_proj layer. */
   int32_t apply_lm_mask;
+  /* 1: apply each level's ResNet dropout (the module is in training mode; independent of save_for_backward).
+   * Element i of the [level_batch][H][W][C] output of a ResNet's SiLU(norm2) is kept when Philox4x32-10 with
+   * key = dropout_seed and counter = (i / 4, stream id) gives a word w (word i % 4) with w / 2^32 >= p; the stream id
+   * is the mdm_net_param_info index of that ResNet's conv2.weight. mdm_op_dropout_mask rebuilds a mask. The backward
+   * regenerates the masks of the forward it follows. */
+  int32_t dropout;
+  uint64_t dropout_seed;
 } mdm_net_io;
 
 /* CUDA-graph execution of forward / backward (off by default). With it on, the first call with a given shape
- * signature (batch, per-level batch, resolutions, tokens, mask/micro presence, save_for_backward) runs eagerly, the
+ * signature (batch, per-level batch, resolutions, tokens, mask/micro presence, save_for_backward, dropout) runs
+ * eagerly, the
  * second is captured and later ones replay the captured graphs: inputs / output gradients are copied into static
  * buffers, ONE graph launch runs the ~1-2.5 k kernels of the pass, outputs are copied out. Gradient-ready
  * notifications (mdm_net_set_grad_ready) keep working: the backward is then recorded as one graph per reported range
@@ -332,6 +343,11 @@ int mdm_op_attention_fwd(const void* qkv16, const void* kv16, const float* mask,
 int mdm_op_attention_bwd(const void* qkv16, const void* kv16, const float* mask, const void* dO16, const void* h16,
                          const void* oself16, const float* stats, int B, int T, int S, int C, int heads, float* Dterm,
                          float* dq32, void* dqkv16, void* dkv16, mdm_stream_t stream);
+
+/* ---------------------------------------------------------------- ResNet dropout mask (single operator, for tests)
+ * out_f32[i] (i < n) = the factor the fused GroupNorm kernels apply to element i of a ResNet with this stream id under
+ * this seed (mdm_net_io.dropout): 1/(1-p) when kept, else 0 (always 0 for p == 1). p in [0, 1]. */
+int mdm_op_dropout_mask(uint64_t seed, uint32_t stream_id, int64_t n, float p, float* out_f32, mdm_stream_t stream);
 
 /* ---------------------------------------------------------------- token self-attention (single operator, for tests)
  * SelfAttention1D.attention of the lm_head layers (models/unet.py:350-375): qkv16 (B*T, 3D) fp16 = [q|k|v] thirds,

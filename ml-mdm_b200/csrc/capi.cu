@@ -94,6 +94,21 @@ int mdm_gemm_raw_split(const mdm_tmap_spec* A, const mdm_tmap_spec* B, int a_mn,
   return 0;
 }
 
+int mdm_op_dropout_mask(uint64_t seed, uint32_t stream_id, int64_t n, float p, float* out_f32, mdm_stream_t stream) {
+  if (!(p >= 0.f && p <= 1.f) || n < 0 || (n > 0 && out_f32 == nullptr)) {
+    mdm::set_error("mdm_op_dropout_mask: p must lie in [0, 1], n >= 0 and out_f32 non-null");
+    return -1;
+  }
+  if (n == 0) return 0;
+  mdm::dropout_mask(seed, stream_id, n, p, out_f32, static_cast<cudaStream_t>(stream));
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    mdm::set_error("mdm_op_dropout_mask: %s", cudaGetErrorString(e));
+    return -1;
+  }
+  return 0;
+}
+
 int mdm_gemm_raw(const mdm_tmap_spec* A, const mdm_tmap_spec* B, int a_mn, int b_mn,
                  const mdm_gemm_params* p, mdm_stream_t stream) {
   return mdm_gemm_raw_split(A, B, a_mn, b_mn, p, nullptr, nullptr, stream);

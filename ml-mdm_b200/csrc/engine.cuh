@@ -122,6 +122,9 @@ struct Engine {
   float* d_scale = nullptr;
   float* d_inv_scale = nullptr;
   float* d_amax = nullptr;
+  // seed of the ResNet dropout masks (kernels.cuh Dropout): written on the caller's stream by every forward that
+  // drops, read by the kernels, so a replayed graph draws fresh masks and its backward regenerates the same ones
+  unsigned long long* d_drop_seed = nullptr;
 
   // ---- side stream for weight gradients. A weight gradient feeds nothing else in the step, so its kernels (the
   // wgrad GEMM, its memset and un-pack) can run beside the data-gradient / GroupNorm-backward chain of the same layer

@@ -3,6 +3,7 @@
 
 #include "kernels.cuh"
 
+#include <curand_philox4x32_x.h>  // Philox4x32-10 of curand_kernel.h, header only
 #include <math.h>
 
 #include <algorithm>
@@ -94,6 +95,40 @@ __device__ __forceinline__ void st_half4(__half* p, float a, float b, float c, f
 __device__ __forceinline__ float f16_rest(float a) { return a - __half2float(__float2half_rn(a)); }
 __device__ __forceinline__ void st_half4_lo(__half* p, float a, float b, float c, float d) {
   st_half4(p, f16_rest(a), f16_rest(b), f16_rest(c), f16_rest(d));
+}
+
+// Dropout (kernels.cuh) as the kernels see it: one Philox4x32-10 call gives the four factors of a float4 channel lane.
+struct DropK {
+  const unsigned long long* seed;
+  uint32_t stream;
+  uint32_t thresh;  // keep when the Philox word >= ceil(p * 2^32)
+  float scale;      // 1/(1-p); 0 when p == 1
+};
+DropK drop_k(const Dropout& d) {
+  DropK k{d.seed, d.stream, 0u, 0.f};
+  if (d.p >= 1.f) {
+    k.thresh = 0xffffffffu;
+  } else {
+    k.thresh = static_cast<uint32_t>(std::min(ceil(static_cast<double>(d.p) * 4294967296.0), 4294967295.0));
+    k.scale = static_cast<float>(1.0 / (1.0 - static_cast<double>(d.p)));
+  }
+  return k;
+}
+// factors of elements 4q .. 4q+3
+__device__ __forceinline__ float4 drop_factors(unsigned long long seed, uint32_t stream, uint32_t thresh, float scale,
+                                               long long q) {
+  const uint4 r = curand_Philox4x32_10(
+      make_uint4(static_cast<uint32_t>(q), static_cast<uint32_t>(static_cast<unsigned long long>(q) >> 32), stream, 0u),
+      make_uint2(static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32)));
+  return make_float4(r.x >= thresh ? scale : 0.f, r.y >= thresh ? scale : 0.f, r.z >= thresh ? scale : 0.f,
+                     r.w >= thresh ? scale : 0.f);
+}
+__device__ __forceinline__ float4 drop_factors(const DropK& d, unsigned long long seed, long long q) {
+  return drop_factors(seed, d.stream, d.thresh, d.scale, q);
+}
+template <bool DROP>
+__device__ __forceinline__ unsigned long long drop_seed(const DropK& d) {
+  return DROP ? __ldg(d.seed) : 0ull;
 }
 
 
@@ -358,11 +393,11 @@ __device__ __forceinline__ void gn_coefs(GnCoef<NL>& k, const LaneMap& m, int n,
   }
 }
 
-template <int NL>
+template <int NL, bool DROP>
 __global__ void __launch_bounds__(TPB)
 gn_apply_kernel(Src2 x, int HW, int G, const float* __restrict__ sums, const float* __restrict__ gamma,
                 const float* __restrict__ beta, const float* __restrict__ film, int film_ld, int film_off,
-                int silu, __half* __restrict__ y16, __half* __restrict__ raw16) {
+                int silu, __half* __restrict__ y16, __half* __restrict__ raw16, DropK drop) {
   const int C = x.c0 + x.c1;
   const LaneMap m = lane_map(C);
   const int n = blockIdx.y;
@@ -370,6 +405,7 @@ gn_apply_kernel(Src2 x, int HW, int G, const float* __restrict__ sums, const flo
   const int p_begin = blockIdx.x * per;
   const int p_end = min(HW, p_begin + per);
   if (!m.active) return;
+  const unsigned long long seed = drop_seed<DROP>(drop);
   GnCoef<NL> k;
   gn_coefs(k, m, n, C, G, HW, sums, gamma, beta, film, film_ld, film_off);
   constexpr int U = PixUnroll<NL>::U;
@@ -401,6 +437,10 @@ gn_apply_kernel(Src2 x, int HW, int G, const float* __restrict__ sums, const flo
         if (silu) {
           u0 = siluf_(u0); u1 = siluf_(u1); u2 = siluf_(u2); u3 = siluf_(u3);
         }
+        if (DROP) {
+          const float4 f = drop_factors(drop, seed, pix * m.lanes + l);
+          u0 *= f.x; u1 *= f.y; u2 *= f.z; u3 *= f.w;
+        }
         st_half4(y16 + pix * C + 4 * l, u0, u1, u2, u3);
         if (raw16 != nullptr) st_half4(raw16 + pix * C + 4 * l, v.x, v.y, v.z, v.w);
       }
@@ -409,12 +449,12 @@ gn_apply_kernel(Src2 x, int HW, int G, const float* __restrict__ sums, const flo
   }
 }
 
-template <int NL, bool DY16>
+template <int NL, bool DY16, bool DROP>
 __global__ void __launch_bounds__(TPB)
 gn_bwd_reduce_kernel(Src2 x, const void* __restrict__ dy, int HW, int G, const float* __restrict__ sums,
                      const float* __restrict__ gamma, const float* __restrict__ beta,
                      const float* __restrict__ film, int film_ld, int film_off, int silu,
-                     float* __restrict__ ab) {
+                     float* __restrict__ ab, DropK drop) {
   const int C = x.c0 + x.c1;
   const LaneMap m = lane_map(C);
   const int n = blockIdx.y;
@@ -422,6 +462,7 @@ gn_bwd_reduce_kernel(Src2 x, const void* __restrict__ dy, int HW, int G, const f
   const int p_begin = blockIdx.x * per;
   const int p_end = min(HW, p_begin + per);
   __shared__ float4 red[TPB];
+  const unsigned long long seed = drop_seed<DROP>(drop);
   GnCoef<NL> k;
   if (m.active) gn_coefs(k, m, n, C, G, HW, sums, gamma, beta, film, film_ld, film_off);
   float4 A[NL], Bq[NL];
@@ -454,7 +495,11 @@ gn_bwd_reduce_kernel(Src2 x, const void* __restrict__ dy, int HW, int G, const f
         const int l = m.t_lane + j * m.stride;
         if (l < m.lanes) {
           const float4 v = vv[u][j];
-          const float4 d = dd[u][j];
+          float4 d = dd[u][j];
+          if (DROP) {
+            const float4 f = drop_factors(drop, seed, (static_cast<long long>(n) * HW + p0 + u * m.ppi) * m.lanes + l);
+            d.x *= f.x; d.y *= f.y; d.z *= f.z; d.w *= f.w;
+          }
           const float xh[4] = {v.x * k.rs[j].x + k.nm[j].x, v.y * k.rs[j].y + k.nm[j].y,
                                v.z * k.rs[j].z + k.nm[j].z, v.w * k.rs[j].w + k.nm[j].w};
           const float ga[4] = {k.ga[j].x, k.ga[j].y, k.ga[j].z, k.ga[j].w};
@@ -487,12 +532,12 @@ gn_bwd_reduce_kernel(Src2 x, const void* __restrict__ dy, int HW, int G, const f
 }
 
 
-template <int NL, bool DY16>
+template <int NL, bool DY16, bool DROP>
 __global__ void __launch_bounds__(TPB)
 gn_bwd_reduce_staged_kernel(Src2 x, const void* __restrict__ dy, int HW, int G, const float* __restrict__ sums,
                             const float* __restrict__ gamma, const float* __restrict__ beta,
                             const float* __restrict__ film, int film_ld, int film_off, int silu,
-                            float* __restrict__ ab, int pix, int stage_bytes) {
+                            float* __restrict__ ab, int pix, int stage_bytes, DropK drop) {
   extern __shared__ __align__(128) uint8_t rs_mem[];
   __shared__ __align__(8) uint64_t full[RS_STAGES];
   __shared__ float4 red[TPB];
@@ -515,6 +560,7 @@ gn_bwd_reduce_staged_kernel(Src2 x, const void* __restrict__ dy, int HW, int G, 
       rs.issue(it, x, dy, base_pix + p_begin + it * pix, min(pix, p_end - p_begin - it * pix));
   GnCoef<NL> k;
   if (m.active) gn_coefs(k, m, n, C, G, HW, sums, gamma, beta, film, film_ld, film_off);
+  const unsigned long long seed = drop_seed<DROP>(drop);
   float4 A[NL], Bq[NL];
 #pragma unroll
   for (int j = 0; j < NL; ++j) {
@@ -533,7 +579,11 @@ gn_bwd_reduce_staged_kernel(Src2 x, const void* __restrict__ dy, int HW, int G, 
           const int l = m.t_lane + j * m.stride;
           if (l < m.lanes) {
             const float4 v = rs_ld_x(st, x, pl, 4 * l);
-            const float4 d = rs_ld_dy<DY16>(st, C, pl, 4 * l);
+            float4 d = rs_ld_dy<DY16>(st, C, pl, 4 * l);
+            if (DROP) {
+              const float4 f = drop_factors(drop, seed, (base_pix + p_begin + it * pix + pl) * m.lanes + l);
+              d.x *= f.x; d.y *= f.y; d.z *= f.z; d.w *= f.w;
+            }
             const float xh[4] = {v.x * k.rs[j].x + k.nm[j].x, v.y * k.rs[j].y + k.nm[j].y,
                                  v.z * k.rs[j].z + k.nm[j].z, v.w * k.rs[j].w + k.nm[j].w};
             const float ga[4] = {k.ga[j].x, k.ga[j].y, k.ga[j].z, k.ga[j].w};
@@ -608,12 +658,12 @@ __global__ void gn_bwd_finalize_kernel(int C, int G, int HW, const float* __rest
   }
 }
 
-template <int NL, bool DY16>
+template <int NL, bool DY16, bool DROP>
 __global__ void __launch_bounds__(TPB)
 gn_bwd_apply_kernel(Src2 x, const void* __restrict__ dy, int HW, int G, const float* __restrict__ sums,
                     const float* __restrict__ gamma, const float* __restrict__ beta,
                     const float* __restrict__ film, int film_ld, int film_off, int silu,
-                    const float* __restrict__ pg, const float* __restrict__ extra, Dst2 dst) {
+                    const float* __restrict__ pg, const float* __restrict__ extra, Dst2 dst, DropK drop) {
   const int C = x.c0 + x.c1;
   const int cpg = C / G;
   const LaneMap m = lane_map(C);
@@ -622,6 +672,7 @@ gn_bwd_apply_kernel(Src2 x, const void* __restrict__ dy, int HW, int G, const fl
   const int p_begin = blockIdx.x * per;
   const int p_end = min(HW, p_begin + per);
   __shared__ float4 red[TPB];
+  const unsigned long long seed = drop_seed<DROP>(drop);
   GnCoef<NL> k;
   if (m.active) gn_coefs(k, m, n, C, G, HW, sums, gamma, beta, film, film_ld, film_off);
   float4 csum[NL];
@@ -672,7 +723,11 @@ gn_bwd_apply_kernel(Src2 x, const void* __restrict__ dy, int HW, int G, const fl
       if (l < m.lanes) {
         const int c = 4 * l;
         const float4 v = vv[u][j];
-        const float4 d = dd[u][j];
+        float4 d = dd[u][j];
+        if (DROP) {
+          const float4 f = drop_factors(drop, seed, pix * m.lanes + l);
+          d.x *= f.x; d.y *= f.y; d.z *= f.z; d.w *= f.w;
+        }
         const float xh[4] = {v.x * k.rs[j].x + k.nm[j].x, v.y * k.rs[j].y + k.nm[j].y,
                              v.z * k.rs[j].z + k.nm[j].z, v.w * k.rs[j].w + k.nm[j].w};
         const float ga[4] = {k.ga[j].x, k.ga[j].y, k.ga[j].z, k.ga[j].w};
@@ -734,13 +789,13 @@ gn_bwd_apply_kernel(Src2 x, const void* __restrict__ dy, int HW, int G, const fl
 }
 
 
-template <int NL, bool DY16>
+template <int NL, bool DY16, bool DROP>
 __global__ void __launch_bounds__(TPB)
 gn_bwd_apply_staged_kernel(Src2 x, const void* __restrict__ dy, int HW, int G, const float* __restrict__ sums,
                            const float* __restrict__ gamma, const float* __restrict__ beta,
                            const float* __restrict__ film, int film_ld, int film_off, int silu,
                            const float* __restrict__ pg, const float* __restrict__ extra, Dst2 dst, int pix,
-                           int stage_bytes) {
+                           int stage_bytes, DropK drop) {
   extern __shared__ __align__(128) uint8_t rs_mem[];
   __shared__ __align__(8) uint64_t full[RS_STAGES];
   __shared__ float4 red[TPB];
@@ -764,6 +819,7 @@ gn_bwd_apply_staged_kernel(Src2 x, const void* __restrict__ dy, int HW, int G, c
       rs.issue(it, x, dy, base_pix + p_begin + it * pix, min(pix, p_end - p_begin - it * pix));
   GnCoef<NL> k;
   if (m.active) gn_coefs(k, m, n, C, G, HW, sums, gamma, beta, film, film_ld, film_off);
+  const unsigned long long seed = drop_seed<DROP>(drop);
   float4 csum[NL], q1[NL], q2[NL];
   const float inv_m = 1.0f / (static_cast<float>(HW) * cpg);
 #pragma unroll
@@ -796,7 +852,11 @@ gn_bwd_apply_staged_kernel(Src2 x, const void* __restrict__ dy, int HW, int G, c
           if (l < m.lanes) {
             const int c = 4 * l;
             const float4 v = rs_ld_x(st, x, pl, c);
-            const float4 d = rs_ld_dy<DY16>(st, C, pl, c);
+            float4 d = rs_ld_dy<DY16>(st, C, pl, c);
+            if (DROP) {
+              const float4 f = drop_factors(drop, seed, gpix * m.lanes + l);
+              d.x *= f.x; d.y *= f.y; d.z *= f.z; d.w *= f.w;
+            }
             const float xh[4] = {v.x * k.rs[j].x + k.nm[j].x, v.y * k.rs[j].y + k.nm[j].y,
                                  v.z * k.rs[j].z + k.nm[j].z, v.w * k.rs[j].w + k.nm[j].w};
             const float ga[4] = {k.ga[j].x, k.ga[j].y, k.ga[j].z, k.ga[j].w};
@@ -976,11 +1036,12 @@ cast_colsum_staged_kernel(const float* __restrict__ in, __half* __restrict__ out
 }
 
 // staged GroupNorm (+FiLM, +SiLU) apply
-template <int NL>
+template <int NL, bool DROP>
 __global__ void __launch_bounds__(TPB)
 gn_apply_staged_kernel(Src2 x, int HW, int G, const float* __restrict__ sums, const float* __restrict__ gamma,
                        const float* __restrict__ beta, const float* __restrict__ film, int film_ld, int film_off,
-                       int silu, __half* __restrict__ y16, __half* __restrict__ raw16, int pix, int stage_bytes) {
+                       int silu, __half* __restrict__ y16, __half* __restrict__ raw16, int pix, int stage_bytes,
+                       DropK drop) {
   extern __shared__ __align__(128) uint8_t rs_mem[];
   __shared__ __align__(8) uint64_t full[RS_STAGES];
   const int C = x.c0 + x.c1;
@@ -1002,6 +1063,7 @@ gn_apply_staged_kernel(Src2 x, int HW, int G, const float* __restrict__ sums, co
       rs.issue(it, x, nullptr, base_pix + p_begin + it * pix, min(pix, p_end - p_begin - it * pix));
   GnCoef<NL> k;
   if (m.active) gn_coefs(k, m, n, C, G, HW, sums, gamma, beta, film, film_ld, film_off);
+  const unsigned long long seed = drop_seed<DROP>(drop);
   for (int it = 0; it < nchunks; ++it) {
     const int s = it % RS_STAGES;
     rs_wait(&full[s], static_cast<uint32_t>(it / RS_STAGES) & 1u);
@@ -1022,6 +1084,10 @@ gn_apply_staged_kernel(Src2 x, int HW, int G, const float* __restrict__ sums, co
             if (silu) {
               u0 = siluf_(u0); u1 = siluf_(u1); u2 = siluf_(u2); u3 = siluf_(u3);
             }
+            if (DROP) {
+              const float4 f = drop_factors(drop, seed, gpix * m.lanes + l);
+              u0 *= f.x; u1 *= f.y; u2 *= f.z; u3 *= f.w;
+            }
             st_half4(y16 + gpix * C + 4 * l, u0, u1, u2, u3);
             if (raw16 != nullptr) st_half4(raw16 + gpix * C + 4 * l, v.x, v.y, v.z, v.w);
           }
@@ -1034,6 +1100,22 @@ gn_apply_staged_kernel(Src2 x, int HW, int G, const float* __restrict__ sums, co
   }
 }
 
+
+__global__ void dropout_set_seed_kernel(unsigned long long* slot, unsigned long long seed) { *slot = seed; }
+
+__global__ void __launch_bounds__(TPB)
+dropout_mask_kernel(unsigned long long seed, uint32_t stream, uint32_t thresh, float scale, long long n,
+                    float* __restrict__ out) {
+  const long long nq = cdiv(n, 4);
+  for (long long q = blockIdx.x * static_cast<long long>(TPB) + threadIdx.x; q < nq;
+       q += static_cast<long long>(gridDim.x) * TPB) {
+    const float4 f = drop_factors(seed, stream, thresh, scale, q);
+    const float fv[4] = {f.x, f.y, f.z, f.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+      if (4 * q + e < n) out[4 * q + e] = fv[e];
+  }
+}
 
 // Column sums of an fp16 matrix (bias gradients of the linear layers): 8 channels (one 16-byte load) per thread and
 // 8 rows in flight per trip. The generic cast_colsum path moved 8 bytes per load, far below the HBM rate on the
@@ -1775,51 +1857,80 @@ void gn_stats(const Src2& x, int N, int HW, int G, float* sums, cudaStream_t st)
   MDM_DISPATCH_NL(C, (gn_stats_kernel<NL><<<grid, TPB, 0, st>>>(x, HW, G, sums)));
   MDM_LAUNCHED();
 }
+// DROP: the kernels' dropout form, for a Dropout with p > 0 (p == 0 takes the plain instantiation)
+#define MDM_DISPATCH_DROP(drop, ...)   \
+  do {                                 \
+    if ((drop).p > 0.f) {              \
+      constexpr bool DROP = true;      \
+      __VA_ARGS__;                     \
+    } else {                           \
+      constexpr bool DROP = false;     \
+      __VA_ARGS__;                     \
+    }                                  \
+  } while (0)
+
+void dropout_set_seed(unsigned long long* slot, unsigned long long seed, cudaStream_t st) {
+  dropout_set_seed_kernel<<<1, 1, 0, st>>>(slot, seed);
+  MDM_LAUNCHED();
+}
+void dropout_mask(unsigned long long seed, uint32_t stream, long long n, float p, float* out, cudaStream_t st) {
+  Dropout d;
+  d.p = p;
+  const DropK k = drop_k(d);
+  dropout_mask_kernel<<<grid_for(cdiv(n, 4), TPB, 132 * 8), TPB, 0, st>>>(seed, stream, k.thresh, k.scale, n, out);
+  MDM_LAUNCHED();
+}
+
 void gn_apply(const Src2& x, int N, int HW, int G, const float* sums, const float* gamma, const float* beta,
               const float* film, int film_ld, int film_off, int silu, __half* y16, __half* raw16,
-              cudaStream_t st) {
+              cudaStream_t st, const Dropout& drop) {
   const int C = x.c0 + x.c1;
+  const DropK dk = drop_k(drop);
   static const bool staged_apply = getenv("MDM_APPLY_LEGACY") == nullptr;
   if (g_gn_staged && staged_apply && (x.c0 % 4 == 0) && (x.c1 % 4 == 0) && (C % 8 == 0)) {
     int pix, sb;
     rs_geometry(C, 0, &pix, &sb);
     const int smem = RS_STAGES * sb;
     dim3 grid(staged_chunks(N, HW, pix, smem), N);
-    MDM_DISPATCH_NL(C, MDM_LAUNCH_STAGED((gn_apply_staged_kernel<NL>), grid, smem, x, HW, G, sums, gamma, beta, film, film_ld,
-                                         film_off, silu, y16, raw16, pix, sb));
+    MDM_DISPATCH_DROP(drop, MDM_DISPATCH_NL(C, MDM_LAUNCH_STAGED((gn_apply_staged_kernel<NL, DROP>), grid, smem, x, HW, G,
+                                                                 sums, gamma, beta, film, film_ld, film_off, silu, y16,
+                                                                 raw16, pix, sb, dk)));
     MDM_LAUNCHED();
     return;
   }
   dim3 grid(pixel_chunks(N, HW, host_ppi(C)), N);
-  MDM_DISPATCH_NL(C, (gn_apply_kernel<NL><<<grid, TPB, 0, st>>>(x, HW, G, sums, gamma, beta, film, film_ld, film_off, silu,
-                                                                y16, raw16)));
+  MDM_DISPATCH_DROP(drop, MDM_DISPATCH_NL(C, (gn_apply_kernel<NL, DROP><<<grid, TPB, 0, st>>>(
+                                                 x, HW, G, sums, gamma, beta, film, film_ld, film_off, silu, y16, raw16, dk))));
   MDM_LAUNCHED();
 }
 void gn_bwd_reduce(const Src2& x, const void* dy, int dy_f16, int N, int HW, int G, const float* sums,
                    const float* gamma, const float* beta, const float* film, int film_ld, int film_off, int silu,
-                   float* ab, cudaStream_t st) {
+                   float* ab, cudaStream_t st, const Dropout& drop) {
   const int C = x.c0 + x.c1;
+  const DropK dk = drop_k(drop);
   if (g_gn_staged && (x.c0 % 4 == 0) && (x.c1 % 4 == 0) && (C % 8 == 0)) {
     int pix, sb;
     rs_geometry(C, dy_f16 ? 2 : 4, &pix, &sb);
     const int smem = RS_STAGES * sb;
     dim3 grid(staged_chunks(N, HW, pix, smem), N);
     if (dy_f16)
-      MDM_DISPATCH_NL(C, MDM_LAUNCH_STAGED((gn_bwd_reduce_staged_kernel<NL, true>), grid, smem, x, dy, HW, G, sums, gamma, beta,
-                                           film, film_ld, film_off, silu, ab, pix, sb));
+      MDM_DISPATCH_DROP(drop, MDM_DISPATCH_NL(C, MDM_LAUNCH_STAGED((gn_bwd_reduce_staged_kernel<NL, true, DROP>), grid, smem,
+                                                                   x, dy, HW, G, sums, gamma, beta, film, film_ld, film_off,
+                                                                   silu, ab, pix, sb, dk)));
     else
-      MDM_DISPATCH_NL(C, MDM_LAUNCH_STAGED((gn_bwd_reduce_staged_kernel<NL, false>), grid, smem, x, dy, HW, G, sums, gamma,
-                                           beta, film, film_ld, film_off, silu, ab, pix, sb));
+      MDM_DISPATCH_DROP(drop, MDM_DISPATCH_NL(C, MDM_LAUNCH_STAGED((gn_bwd_reduce_staged_kernel<NL, false, DROP>), grid, smem,
+                                                                   x, dy, HW, G, sums, gamma, beta, film, film_ld, film_off,
+                                                                   silu, ab, pix, sb, dk)));
     MDM_LAUNCHED();
     return;
   }
   dim3 grid(pixel_chunks(N, HW, host_ppi(C)), N);
   if (dy_f16)
-    MDM_DISPATCH_NL(C, (gn_bwd_reduce_kernel<NL, true><<<grid, TPB, 0, st>>>(x, dy, HW, G, sums, gamma, beta, film, film_ld,
-                                                                             film_off, silu, ab)));
+    MDM_DISPATCH_DROP(drop, MDM_DISPATCH_NL(C, (gn_bwd_reduce_kernel<NL, true, DROP><<<grid, TPB, 0, st>>>(
+                                                   x, dy, HW, G, sums, gamma, beta, film, film_ld, film_off, silu, ab, dk))));
   else
-    MDM_DISPATCH_NL(C, (gn_bwd_reduce_kernel<NL, false><<<grid, TPB, 0, st>>>(x, dy, HW, G, sums, gamma, beta, film,
-                                                                              film_ld, film_off, silu, ab)));
+    MDM_DISPATCH_DROP(drop, MDM_DISPATCH_NL(C, (gn_bwd_reduce_kernel<NL, false, DROP><<<grid, TPB, 0, st>>>(
+                                                   x, dy, HW, G, sums, gamma, beta, film, film_ld, film_off, silu, ab, dk))));
   MDM_LAUNCHED();
 }
 void gn_bwd_finalize(int N, int C, int G, int HW, const float* ab, const float* gamma, const float* beta,
@@ -1831,29 +1942,34 @@ void gn_bwd_finalize(int N, int C, int G, int HW, const float* ab, const float* 
 }
 void gn_bwd_apply(const Src2& x, const void* dy, int dy_f16, int N, int HW, int G, const float* sums,
                   const float* gamma, const float* beta, const float* film, int film_ld, int film_off, int silu,
-                  const float* pg, const float* extra, const Dst2& dst, cudaStream_t st) {
+                  const float* pg, const float* extra, const Dst2& dst, cudaStream_t st, const Dropout& drop) {
   const int C = x.c0 + x.c1;
+  const DropK dk = drop_k(drop);
   if (g_gn_staged && (x.c0 % 4 == 0) && (x.c1 % 4 == 0) && (C % 8 == 0)) {
     int pix, sb;
     rs_geometry(C, dy_f16 ? 2 : 4, &pix, &sb);
     const int smem = RS_STAGES * sb;
     dim3 grid(staged_chunks(N, HW, pix, smem), N);
     if (dy_f16)
-      MDM_DISPATCH_NL(C, MDM_LAUNCH_STAGED((gn_bwd_apply_staged_kernel<NL, true>), grid, smem, x, dy, HW, G, sums, gamma, beta,
-                                           film, film_ld, film_off, silu, pg, extra, dst, pix, sb));
+      MDM_DISPATCH_DROP(drop, MDM_DISPATCH_NL(C, MDM_LAUNCH_STAGED((gn_bwd_apply_staged_kernel<NL, true, DROP>), grid, smem,
+                                                                   x, dy, HW, G, sums, gamma, beta, film, film_ld, film_off,
+                                                                   silu, pg, extra, dst, pix, sb, dk)));
     else
-      MDM_DISPATCH_NL(C, MDM_LAUNCH_STAGED((gn_bwd_apply_staged_kernel<NL, false>), grid, smem, x, dy, HW, G, sums, gamma,
-                                           beta, film, film_ld, film_off, silu, pg, extra, dst, pix, sb));
+      MDM_DISPATCH_DROP(drop, MDM_DISPATCH_NL(C, MDM_LAUNCH_STAGED((gn_bwd_apply_staged_kernel<NL, false, DROP>), grid, smem,
+                                                                   x, dy, HW, G, sums, gamma, beta, film, film_ld, film_off,
+                                                                   silu, pg, extra, dst, pix, sb, dk)));
     MDM_LAUNCHED();
     return;
   }
   dim3 grid(pixel_chunks(N, HW, host_ppi(C)), N);
   if (dy_f16)
-    MDM_DISPATCH_NL(C, (gn_bwd_apply_kernel<NL, true><<<grid, TPB, 0, st>>>(x, dy, HW, G, sums, gamma, beta, film, film_ld,
-                                                                            film_off, silu, pg, extra, dst)));
+    MDM_DISPATCH_DROP(drop, MDM_DISPATCH_NL(C, (gn_bwd_apply_kernel<NL, true, DROP><<<grid, TPB, 0, st>>>(
+                                                   x, dy, HW, G, sums, gamma, beta, film, film_ld, film_off, silu, pg, extra,
+                                                   dst, dk))));
   else
-    MDM_DISPATCH_NL(C, (gn_bwd_apply_kernel<NL, false><<<grid, TPB, 0, st>>>(x, dy, HW, G, sums, gamma, beta, film,
-                                                                             film_ld, film_off, silu, pg, extra, dst)));
+    MDM_DISPATCH_DROP(drop, MDM_DISPATCH_NL(C, (gn_bwd_apply_kernel<NL, false, DROP><<<grid, TPB, 0, st>>>(
+                                                   x, dy, HW, G, sums, gamma, beta, film, film_ld, film_off, silu, pg, extra,
+                                                   dst, dk))));
   MDM_LAUNCHED();
 }
 

@@ -28,18 +28,33 @@ struct Dst2 {
   __half* h16lo;  // optional second fp16 plane of h16: fp16(v - h16)
 };
 
+// ---- dropout on the output of a GroupNorm apply (ResNet.dropout, reference unet.py:208,233-235)
+// Element i (NHWC linear index of the [N][HW][C] output) is kept when u >= p, where u * 2^32 is word i % 4 of
+// Philox4x32-10 with key = *seed and counter = (i / 4 as two words, stream, 0); kept elements are scaled by 1/(1-p) and
+// p == 1 drops everything. The mask is a pure function of (seed, stream, i): the backward regenerates it.
+struct Dropout {
+  float p = 0.f;                           // 0: off (the kernels take their plain form)
+  const unsigned long long* seed = nullptr;  // device slot, read by the kernels (a replayed graph sees its new value)
+  uint32_t stream = 0;
+};
+// *slot = seed, one thread on st (no host synchronisation)
+void dropout_set_seed(unsigned long long* slot, unsigned long long seed, cudaStream_t st);
+// out[i] = the factor (0 or 1/(1-p)) the fused kernels apply to element i, i < n
+void dropout_mask(unsigned long long seed, uint32_t stream, long long n, float p, float* out, cudaStream_t st);
+
 // ---- GroupNorm family (reference: nn.GroupNorm(32, C) in unet.py:198,207,259,268,749)
 // sums: [N][G][2] (sum, sumsq), must be zero on entry.
 void gn_stats(const Src2& x, int N, int HW, int G, float* sums, cudaStream_t st);
-// y16 = act(gn(x) * (1 + ta) + tb); film = [N][film_ld] fp32 rows with ta at film_off, tb at
+// y16 = drop(act(gn(x) * (1 + ta) + tb)); film = [N][film_ld] fp32 rows with ta at film_off, tb at
 // film_off + C (null: no FiLM). raw16 (optional) receives the un-normalised fp16 copy of x.
 void gn_apply(const Src2& x, int N, int HW, int G, const float* sums, const float* gamma,
               const float* beta, const float* film, int film_ld, int film_off, int silu, __half* y16,
-              __half* raw16, cudaStream_t st);
-// Backward. dy: fp32 or fp16 (dy_f16) [N][HW][C] gradient w.r.t. y16.  ab: [N][C][2] scratch, zero on entry.
+              __half* raw16, cudaStream_t st, const Dropout& drop = Dropout());
+// Backward. dy: fp32 or fp16 (dy_f16) [N][HW][C] gradient w.r.t. y16; `drop` as in the forward.
+// ab: [N][C][2] scratch, zero on entry.
 void gn_bwd_reduce(const Src2& x, const void* dy, int dy_f16, int N, int HW, int G, const float* sums,
                    const float* gamma, const float* beta, const float* film, int film_ld, int film_off,
-                   int silu, float* ab, cudaStream_t st);
+                   int silu, float* ab, cudaStream_t st, const Dropout& drop = Dropout());
 // pg: [N][G][2] scratch (written). dgamma/dbeta: += inv_scale * grad. dfilm (optional): dense
 // [N][2C] rows (d_ta | d_tb), overwritten.
 void gn_bwd_finalize(int N, int C, int G, int HW, const float* ab, const float* gamma, const float* beta,
@@ -48,7 +63,8 @@ void gn_bwd_finalize(int N, int C, int G, int HW, const float* ab, const float* 
 // dx = rstd * (du*(1+ta)*gamma - P1/m - xhat*P2/m) + extra ; written/accumulated into dst.
 void gn_bwd_apply(const Src2& x, const void* dy, int dy_f16, int N, int HW, int G, const float* sums,
                   const float* gamma, const float* beta, const float* film, int film_ld, int film_off,
-                  int silu, const float* pg, const float* extra, const Dst2& dst, cudaStream_t st);
+                  int silu, const float* pg, const float* extra, const Dst2& dst, cudaStream_t st,
+                  const Dropout& drop = Dropout());
 
 // ---- precision / reductions
 // out16 = half(in) and colsum[c] += inv_scale * sum_rows(in[:, c]) (colsum may be null).

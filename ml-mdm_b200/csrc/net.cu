@@ -248,6 +248,7 @@ struct Net {
       const bool cond_here = cfg.cond_dim > 0;
       MDM_CHECK(c.num_res >= 1 && c.num_res <= MDM_MAX_RES, "bad num_res");
       MDM_CHECK(td % 8 == 0, "temporal_dim must be a multiple of 8");
+      MDM_CHECK(c.dropout >= 0.f && c.dropout <= 1.f, "dropout must lie in [0, 1]");
       // Parameter registration order follows nn.Module registration order of the reference so that
       // index order == state_dict order.
       add_param(pre + "t_emb", {1, td / 8}, 0);  // non-persistent buffer of the reference (unet.py:600-603)
@@ -365,6 +366,7 @@ struct Net {
     eng.d_inv_scale = eng.d_scale + 1;
     eng.d_amax = eng.d_scale + 2;
     persistent.push_back(eng.d_scale);
+    eng.d_drop_seed = static_cast<unsigned long long*>(persist(sizeof(unsigned long long)));
   }
 
   // ---------------------------------------------------------------- weight packing
@@ -493,7 +495,7 @@ struct Net {
     __half* raw16;
   };
   GnOut gn_fwd(const Src2& x, int N, int HW, int G, Param& gw, Param& gb, const float* film, int film_ld,
-               int film_off, int silu, bool want_raw) {
+               int film_off, int silu, bool want_raw, const Dropout& drop = Dropout()) {
     const int C = x.c0 + x.c1;
     MDM_CHECK(C % G == 0 && C % 4 == 0 && x.c0 % 4 == 0, "GroupNorm channel layout");
     GnOut o;
@@ -501,7 +503,7 @@ struct Net {
     gn_stats(x, N, HW, G, o.sums, eng.st);
     o.y16 = eng.alloc<__half>(static_cast<long long>(N) * HW * C);
     o.raw16 = want_raw ? eng.alloc<__half>(static_cast<long long>(N) * HW * C) : nullptr;
-    gn_apply(x, N, HW, G, o.sums, gw.w, gb.w, film, film_ld, film_off, silu, o.y16, o.raw16, eng.st);
+    gn_apply(x, N, HW, G, o.sums, gw.w, gb.w, film, film_ld, film_off, silu, o.y16, o.raw16, eng.st, drop);
     return o;
   }
   // Backward through gn_apply. dy: gradient w.r.t. its fp16 output, fp16 (dy_f16) or fp32.
@@ -509,11 +511,12 @@ struct Net {
   // tensor plus bias-gradient column sums (single consumer, nothing to accumulate).
   void gn_bwd(const Src2& x, const void* dy, bool dy_f16, int N, int HW, int G, const float* sums, Param& gw, Param& gb,
               const float* film, int film_ld, int film_off, int silu, float* dfilm, const float* extra, Act* dst0,
-              Act* dst1, __half* h16_out = nullptr, float* colsum = nullptr, __half* h16_lo = nullptr) {
+              Act* dst1, __half* h16_out = nullptr, float* colsum = nullptr, __half* h16_lo = nullptr,
+              const Dropout& drop = Dropout()) {
     const int C = x.c0 + x.c1;
     float* ab = eng.zeros_f32(2ll * N * C);
     float* pg = eng.alloc<float>(2ll * N * G);
-    gn_bwd_reduce(x, dy, dy_f16 ? 1 : 0, N, HW, G, sums, gw.w, gb.w, film, film_ld, film_off, silu, ab, eng.st);
+    gn_bwd_reduce(x, dy, dy_f16 ? 1 : 0, N, HW, G, sums, gw.w, gb.w, film, film_ld, film_off, silu, ab, eng.st, drop);
     // dgamma/dbeta always have somewhere to go: when a grad buffer is missing use scratch
     float* dg = gw.g != nullptr ? gw.g : eng.zeros_f32(C);
     float* db = gb.g != nullptr ? gb.g : eng.zeros_f32(C);
@@ -536,7 +539,8 @@ struct Net {
         d.acc1 = a1;
       }
     }
-    gn_bwd_apply(x, dy, dy_f16 ? 1 : 0, N, HW, G, sums, gw.w, gb.w, film, film_ld, film_off, silu, pg, extra, d, eng.st);
+    gn_bwd_apply(x, dy, dy_f16 ? 1 : 0, N, HW, G, sums, gw.w, gb.w, film, film_ld, film_off, silu, pg, extra, d, eng.st,
+                 drop);
     eng.rel(ab);
     eng.rel(pg);
   }
@@ -561,7 +565,14 @@ struct Net {
       eng.conv3x3_fwd(g1.y16, cin, N, H, W, cin, c1w.w16, cout, e, c1w.w16f, c1w.bias_f);
     }
     Src2 hs{h, nullptr, cout, 0};
-    GnOut g2 = gn_fwd(hs, N, HW, G, n2w, n2b, ls->film, L.film_total, r.film_off, 1, false);
+    // ResNet.dropout sits between SiLU(norm2) and conv2 (unet.py:233-235); its mask stream is conv2's parameter index
+    Dropout drop;
+    if (io->dropout && L.c.dropout > 0.f) {
+      drop.p = L.c.dropout;
+      drop.seed = eng.d_drop_seed;
+      drop.stream = static_cast<uint32_t>(pindex.at(r.pre + ".conv2.weight"));
+    }
+    GnOut g2 = gn_fwd(hs, N, HW, G, n2w, n2b, ls->film, L.film_total, r.film_off, 1, false, drop);
     const float* res = x->p;
     float* sproj = nullptr;
     if (proj) {
@@ -627,7 +638,7 @@ struct Net {
       __half* dh16lo = E.alloc<__half>(rows * cout);
       float* dfilm = E.alloc<float>(2ll * N * cout);
       gn_bwd(Src2{h, nullptr, cout, 0}, da2, false, N, HW, G, g2.sums, n2w, n2b, ls->film, Lp->film_total, r.film_off, 1,
-             dfilm, nullptr, nullptr, nullptr, dh16, c1b.g, dh16lo);
+             dfilm, nullptr, nullptr, nullptr, dh16, c1b.g, dh16lo, drop);
       E.rel(da2);
       // time layer: film = silu(temb) Wt^T + bt  (batch rows)
       {
@@ -1752,7 +1763,7 @@ struct Net {
   // pool; pool addresses, TMA descriptors and gradient pointers are baked into the graph, so anything that moves them
   // (rebinding parameters, the pool returning memory to the driver) drops the recorded graphs.
   struct GraphRec {
-    int training = 0, batch = 0, tokens = 0, has_mask = 0, has_micro = 0, apply_lm_mask = 0;
+    int training = 0, batch = 0, tokens = 0, has_mask = 0, has_micro = 0, apply_lm_mask = 0, dropout = 0;
     int lb[MDM_MAX_LEVELS] = {0, 0, 0, 0}, res[MDM_MAX_LEVELS] = {0, 0, 0, 0};
     uint64_t bind_epoch = 0, pool_epoch = 0;
     float* x_t[MDM_MAX_LEVELS] = {nullptr, nullptr, nullptr, nullptr};
@@ -1801,7 +1812,7 @@ struct Net {
   }
   bool same_key(const GraphRec& r, const mdm_net_io* q) const {
     if (r.training != (q->save_for_backward != 0) || r.batch != q->batch || r.tokens != q->tokens ||
-        r.apply_lm_mask != (q->apply_lm_mask != 0) ||
+        r.apply_lm_mask != (q->apply_lm_mask != 0) || r.dropout != (q->dropout != 0) ||
         r.has_mask != (q->lm_mask != nullptr) || r.has_micro != (q->micro_scale != nullptr))
       return false;
     for (int l = 0; l < cfg.num_levels; ++l)
@@ -1825,6 +1836,7 @@ struct Net {
     r.has_mask = q->lm_mask != nullptr;
     r.has_micro = q->micro_scale != nullptr;
     r.apply_lm_mask = q->apply_lm_mask != 0;
+    r.dropout = q->dropout != 0;
     for (int l = 0; l < cfg.num_levels; ++l) {
       r.res[l] = q->res[l];
       r.lb[l] = q->level_batch[l] > 0 ? q->level_batch[l] : q->batch;
@@ -1867,6 +1879,8 @@ struct Net {
 
   void forward(const mdm_net_io* io_, cudaStream_t st) {
     active_graph = -1;
+    // on the caller's stream ahead of the eager, captured or replayed pass: the kernels read the seed from its slot
+    if (io_->dropout) dropout_set_seed(eng.d_drop_seed, io_->dropout_seed, st);
     if (!graph_mode || g_profile) {
       forward_body(io_, st);
       return;

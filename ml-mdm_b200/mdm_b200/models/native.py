@@ -25,6 +25,7 @@ class LevelCfg(C.Structure):
         ("skip_normalization", C.c_int32),
         ("has_micro_scale", C.c_int32),
         ("micro_scale_default", C.c_float),
+        ("dropout", C.c_float),
     ]
 
 
@@ -58,6 +59,8 @@ class NetIO(C.Structure):
         ("save_for_backward", C.c_int32),
         ("level_batch", C.c_int32 * MAX_LEVELS),
         ("apply_lm_mask", C.c_int32),
+        ("dropout", C.c_int32),
+        ("dropout_seed", C.c_uint64),
     ]
 
 
@@ -104,6 +107,7 @@ def build_net_cfg(module) -> NetCfg:
         lc.skip_normalization = int(bool(getattr(cfg, "skip_normalization", True)))
         lc.has_micro_scale = int(m.conditions is not None)
         lc.micro_scale_default = float(m.conditions["scale"]) if m.conditions is not None else 0.0
+        lc.dropout = float(cfg.resnet_config.dropout)
     inner = mods[-1]
     icfg = cfgs[-1]
     nc.in_channels = module.input_channels
@@ -186,6 +190,11 @@ class NativeNet:
         self._ready_cb = None
         self._keep = None
         self.apply_lm_mask = False
+        # ResNet dropout: the largest p of the nest, the modules whose train/eval flag it follows, and the
+        # (flag, seed) of the forward being entered
+        self.max_dropout = max(self.cfg.levels[i].dropout for i in range(self.cfg.num_levels))
+        self._dropouts = [m for m in module.modules() if isinstance(m, torch.nn.Dropout)]
+        self.dropout = (0, 0)
         # CUDA-graph replay of forward / backward (mdm_net_set_graph_mode): on unless MDM_NO_GRAPH is set; switched
         # off for this net by gradient accumulation (a fresh arena per backward would re-record every step). With a
         # gradient-ready callback installed the backward is recorded as one graph per reported range.
@@ -275,6 +284,15 @@ class NativeNet:
         micro = None
         if micros:
             micro = micros.get("scale", None)
+        self.dropout = (0, 0)
+        if self.max_dropout > 0:
+            training = self.module.training
+            if any(d.training != training for d in self._dropouts):
+                raise _lib.MdmError("the ResNets' nn.Dropout modules disagree with the model's train/eval mode; the "
+                                    "engine applies dropout to every ResNet or to none (use model.train() / .eval())")
+            if training:
+                # from torch's default CPU generator: reproducible under torch.manual_seed, no device sync
+                self.dropout = (1, int(torch.randint(2**63 - 1, ())))
         # (Function.forward runs with grad mode off, so the decision is taken here)
         need_grad = torch.is_grad_enabled() and any(p.requires_grad for p in self.params)
         return _DenoiseFn.apply(self, len(xs), need_grad, times, lm, mask, micro, *xs, *self.params)
@@ -328,6 +346,7 @@ class NativeNet:
             io.micro_scale = micro.data_ptr()
         io.save_for_backward = int(save)
         io.apply_lm_mask = int(bool(apply_lm_mask))
+        io.dropout, io.dropout_seed = self.dropout
         st = torch.cuda.current_stream().cuda_stream
         _lib.check(self.lib.mdm_net_forward(self.handle, C.byref(io), C.c_void_p(st)), "mdm_net_forward")
         self._keep = keep if save else None  # inputs must outlive the tape

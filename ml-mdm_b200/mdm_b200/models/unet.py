@@ -45,12 +45,14 @@ def _ints(v, n=None):
 class _ResNet(nn.Module):
     """Parameters of one residual unit (reference ResNet, unet.py:193-221)."""
 
-    def __init__(self, temporal_dim, cin, cout, groups):
+    def __init__(self, temporal_dim, cin, cout, groups, dropout):
         super().__init__()
         self.norm1 = nn.GroupNorm(groups, cin)
         self.conv1 = nn.Conv2d(cin, cout, 3, padding=1)
         self.time_layer = nn.Linear(temporal_dim, cout * 2)
         self.norm2 = nn.GroupNorm(groups, cout)
+        # no parameters; carries the train/eval flag the engine's fused dropout follows (native.py)
+        self.dropout = nn.Dropout(dropout)
         self.conv2 = zero_module(nn.Conv2d(cout, cout, 3, padding=1))
         if cin != cout:
             self.conv3 = nn.Conv2d(cin, cout, 1)
@@ -112,9 +114,9 @@ class SelfAttention1DBlock(nn.Module):
 class _Block(nn.Module):
     """Parameters of one resolution block (reference ResNetBlock, unet.py:449-532)."""
 
-    def __init__(self, temporal_dim, res_io, nattn, down, up, cond_dim, groups, use_ffn):
+    def __init__(self, temporal_dim, res_io, nattn, down, up, cond_dim, groups, use_ffn, dropout):
         super().__init__()
-        self.resnets = nn.ModuleList([_ResNet(temporal_dim, ci, co, groups) for ci, co in res_io])
+        self.resnets = nn.ModuleList([_ResNet(temporal_dim, ci, co, groups, dropout) for ci, co in res_io])
         if nattn > 0:
             self.attn = nn.ModuleList(
                 [_Attention(co, cond_dim, use_ffn) for (_, co) in res_io for _ in range(nattn)])
@@ -133,6 +135,7 @@ class UNet(nn.Module):
         rc = config.resnet_config
         groups = rc.num_groups_norm
         use_ffn = bool(rc.use_attention_ffn)
+        dropout = rc.dropout
         channels_list = _ints(config.resolution_channels)
         L = len(channels_list)
         nres = _ints(config.num_resnets_per_resolution, L)
@@ -181,17 +184,19 @@ class UNet(nn.Module):
             if i != L - 1:
                 skips.append(ch)
             na = nattn[i] if i in attn_levels else 0
-            down.append(_Block(td, io, na, i != L - 1, False, cond_dim if i in attn_levels else -1, groups, use_ffn))
+            down.append(_Block(td, io, na, i != L - 1, False, cond_dim if i in attn_levels else -1, groups, use_ffn,
+                               dropout))
         if not config.skip_mid_blocks:
-            mid = [_Block(td, [(ch, ch)], 1, False, False, cond_dim, groups, use_ffn),
-                   _Block(td, [(ch, ch)], 0, False, False, -1, groups, use_ffn)]
+            mid = [_Block(td, [(ch, ch)], 1, False, False, cond_dim, groups, use_ffn, dropout),
+                   _Block(td, [(ch, ch)], 0, False, False, -1, groups, use_ffn, dropout)]
         for i in reversed(range(L)):
             io = []
             for _ in range(nres[i] + 1):
                 io.append((ch + skips.pop(), channels_list[i]))
                 ch = channels_list[i]
             na = nattn[i] if i in attn_levels else 0
-            up.append(_Block(td, io, na, False, i != 0, cond_dim if i in attn_levels else -1, groups, use_ffn))
+            up.append(_Block(td, io, na, False, i != 0, cond_dim if i in attn_levels else -1, groups, use_ffn,
+                             dropout))
         self.norm_out = nn.GroupNorm(groups, ch)
         self.conv_out = zero_module(nn.Conv2d(ch, output_channels, 3, padding=1))
         self.down_blocks = nn.ModuleList(down)
