@@ -188,7 +188,8 @@ typedef struct mdm_net_io {
 } mdm_net_io;
 
 /* CUDA-graph execution of forward / backward (off by default). With it on, the first call with a given shape
- * signature (batch, per-level batch, resolutions, tokens, mask/micro presence, save_for_backward, dropout) runs
+ * signature (batch, per-level batch, resolutions, tokens, mask/micro presence, save_for_backward, dropout, stage,
+ * cond_cache, cond_emb presence; stage-1 calls always run eagerly) runs
  * eagerly, the
  * second is captured and later ones replay the captured graphs: inputs / output gradients are copied into static
  * buffers, ONE graph launch runs the ~1-2.5 k kernels of the pass, outputs are copied out. Gradient-ready
@@ -207,11 +208,45 @@ int mdm_set_sm_reserve(int sms);
 /* UNet.forward / NestedUNet.forward (unet.py:971-987). */
 int mdm_net_forward(mdm_net* net, const mdm_net_io* io, mdm_stream_t stream);
 
+/* The split forward: what mdm_net_forward_stage runs beside the mdm_net_io it is given. A zero-initialised struct (or
+ * NULL) is mdm_net_forward. */
+typedef struct mdm_net_stage_io {
+  /* UNet.forward_conditioning / forward_denoising (unet.py:847-865, 935-969; nested_unet.py:165-230) as separate calls.
+   * 0: both, as mdm_net_forward always did. 1: conditioning only: lm_proj (with apply_lm_mask), the lm_head layers,
+   * the pooled mean (the plain mean with lm_head and unmasked cross-attention, else the masked mean over lm_mask) and
+   * cond_emb; writes cond_out and cond_emb_out and nothing else (x_t / times / out are not read). Its backward
+   * recomputes the text path from the same inputs, so lm / lm_mask must stay valid until then. 2: denoising only:
+   * cond / cond_emb / cross_mask replace the text path; the token LayerNorm and the kv_cond products of the
+   * cross-attention blocks (unet.py:263-264,304) belong to this stage. temb = time MLP + cond_emb + micro. */
+  int32_t stage;
+  float* cond_out;         /* stage 1: (batch, tokens, cond_dim) fp32 */
+  float* cond_emb_out;     /* stage 1: (batch, temporal_dim of the innermost level) fp32; unused without cond_emb */
+  const float* cond;       /* stage 2: (batch, tokens, cond_dim) fp32 (may be NULL with cond_cache 2) */
+  const float* cond_emb;   /* stage 2: (batch, temporal_dim) fp32 or NULL (nothing added to temb) */
+  const float* cross_mask; /* stage 2: (batch, tokens) fp32 0/1 key mask of cross-attention, or NULL */
+  /* Stage 2 without save_for_backward: reuse of the text encoding across calls, one slot per net.
+   * 1: the fp16 K/V every cross-attention block computes from cond are kept in net-owned memory (at fixed addresses,
+   * so replayed graphs read them directly). 2: they are read from there; the token LayerNorm and every kv_cond
+   * product are skipped and cond is not read. Mode 2 fails (nothing runs) unless a mode-1 call with the same batch,
+   * level_batch and tokens filled the slot and neither mdm_net_weights_changed nor mdm_net_bind_param came since.
+   * Whether cond itself is unchanged is the caller's to know. */
+  int32_t cond_cache;
+} mdm_net_stage_io;
+int mdm_net_forward_stage(mdm_net* net, const mdm_net_io* io, const mdm_net_stage_io* stage, mdm_stream_t stream);
+
 typedef struct mdm_net_grad_io {
   const float* dout[MDM_MAX_LEVELS]; /* d loss / d out[l], NCHW fp32; NULL => zero */
+  /* split forward (mdm_net_stage_io.stage). 1: differentiate the last stage-1 forward with save_for_backward=1; otherwise
+   * the last stage-0 / stage-2 one. Each keeps its own saved state, so the two backwards may run in either order. */
+  int32_t stage;
+  float* dcond;              /* stage 2 out: d loss / d cond (batch, tokens, cond_dim) fp32, overwritten; or NULL */
+  float* dcond_emb;          /* stage 2 out: d loss / d cond_emb (batch, temporal_dim) fp32, overwritten; or NULL */
+  const float* dcond_in;     /* stage 1 in: d loss / d cond_out, or NULL (zero) */
+  const float* dcond_emb_in; /* stage 1 in: d loss / d cond_emb_out, or NULL (zero) */
 } mdm_net_grad_io;
 
-/* Backward of the last mdm_net_forward(save_for_backward=1): accumulates parameter gradients. */
+/* Backward of the last mdm_net_forward(save_for_backward=1): accumulates parameter gradients. A split backward
+ * (stage 1 or 2) reports no gradient-ready ranges: its caller reduces the gradients afterwards. */
 int mdm_net_backward(mdm_net* net, const mdm_net_grad_io* gio, mdm_stream_t stream);
 
 /* Overlap of the data-parallel gradient all-reduce with backward (replaces DDP's bucket hooks,
@@ -234,7 +269,8 @@ int mdm_net_grad_order(const mdm_net* net, int32_t* rank, int32_t n);
 uint64_t mdm_net_workspace_bytes(const mdm_net* net);
 uint64_t mdm_net_workspace_high_water(const mdm_net* net);
 /* Debug: copy a named fp32 intermediate of the last forward (e.g. "down_blocks.0.0") to dst.
- * Returns its element count, or negative if unknown. Layout NHWC. */
+ * Returns its element count, or negative if unknown. Layout NHWC. "cond_kv" copies the valid K/V cache
+ * (mdm_net_stage_io.cond_cache) as raw fp16 bits, two per float, in the cache's block-major layout. */
 int64_t mdm_net_debug_fetch(mdm_net* net, const char* name, float* dst, int64_t max_elems, mdm_stream_t stream);
 
 

@@ -127,7 +127,7 @@ void Engine::side_join() {
   MDM_CUDA(cudaEventRecord(e, side));
   MDM_CUDA(cudaStreamWaitEvent(st, e, 0));
   side_active = false;
-  for (void* p : deferred) pool.release(p);
+  for (void* p : deferred) cur_pool().release(p);
   deferred.clear();
 }
 

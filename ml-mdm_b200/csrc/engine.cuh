@@ -101,6 +101,10 @@ struct Epi {
 struct Engine {
   cudaStream_t st = nullptr;
   Pool pool;
+  // while set, alloc / rel draw from this pool instead: the text path of a split forward (net.cu) runs beside a held
+  // tape and must neither reset nor hand out the blocks that tape (or a captured graph) still owns
+  Pool* alt = nullptr;
+  Pool& cur_pool() { return alt != nullptr ? *alt : pool; }
   // Weights are held as two fp16 planes, hi = fp16(w) and lo = fp16(w - hi), in one allocation [hi | lo]; a GEMM whose
   // B operand lies in a hi plane also multiplies the lo plane, so weights enter every product at ~22 significant bits
   // and only the activation operands are rounded to fp16. Key: hi-plane base address, value: plane size (halves).
@@ -154,12 +158,12 @@ struct Engine {
   void rel(void* p) {
     if (p == nullptr) return;
     if (side_active) deferred.push_back(p);
-    else pool.release(p);
+    else cur_pool().release(p);
   }
 
   template <typename T>
   T* alloc(long long n) {
-    return static_cast<T*>(pool.alloc(static_cast<size_t>(n) * sizeof(T)));
+    return static_cast<T*>(cur_pool().alloc(static_cast<size_t>(n) * sizeof(T)));
   }
   float* zeros_f32(long long n);
   Act* new_act(int n, int h, int w, int c, bool alloc_data = true);

@@ -1224,6 +1224,13 @@ __global__ void axpy_f32_kernel(float* __restrict__ dst, const float* __restrict
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
   for (; i < n; i += stride) dst[i] = (acc ? dst[i] : 0.f) + alpha * a[i];
 }
+__global__ void scale_f32_kernel(float* __restrict__ dst, const float* __restrict__ a, const float* __restrict__ s,
+                                 long long n) {
+  const float f = *s;
+  long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  for (; i < n; i += stride) dst[i] = f * a[i];
+}
 
 // ------------------------------------------------------------------ softmax (warp per row)
 __device__ __forceinline__ float warp_max(float v) {
@@ -2030,6 +2037,10 @@ void add_f32(float* dst, const float* a, const float* b, long long n, cudaStream
 }
 void axpy_f32(float* dst, const float* a, float alpha, long long n, int acc, cudaStream_t st) {
   axpy_f32_kernel<<<grid_for(n), 256, 0, st>>>(dst, a, alpha, n, acc);
+  MDM_LAUNCHED();
+}
+void scale_f32(float* dst, const float* a, const float* scale, long long n, cudaStream_t st) {
+  scale_f32_kernel<<<grid_for(n), 256, 0, st>>>(dst, a, scale, n);
   MDM_LAUNCHED();
 }
 

@@ -77,6 +77,7 @@ void cast_f32_to_f16(const float* in, __half* out, long long n, cudaStream_t st)
 void cast_rowscale_f16(const float* in, const float* rowscale, __half* out16, long long rows, int D, cudaStream_t st);
 void add_f32(float* dst, const float* a, const float* b, long long n, cudaStream_t st);  // dst = a + b
 void axpy_f32(float* dst, const float* a, float alpha, long long n, int acc, cudaStream_t st);
+void scale_f32(float* dst, const float* a, const float* scale, long long n, cudaStream_t st);  // dst = *scale * a
 
 // ---- attention pieces (reference unet.py:276-294)
 // P16[r][:] = softmax(scores[r][:]) ; mask (optional) is [B][S] with row r belonging to batch

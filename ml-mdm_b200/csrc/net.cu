@@ -26,6 +26,9 @@ namespace mdm {
 
 unsigned long long g_graph_launches = 0;
 
+// what one forward call is given: the io and the split-forward fields beside it (mdm_net_forward_stage)
+struct StepIO : mdm_net_io, mdm_net_stage_io {};
+
 namespace {
 
 struct ResSpec {
@@ -38,6 +41,7 @@ struct AttnSpec {
   int C;
   bool cond, ffn;
   float* kv_bias_fold = nullptr;  // W b_ln + bias of kv_cond with the LayerNorm affine folded in (persistent)
+  long long kv_col = 0;            // offset of this block's K/V in the cache, in units of batch * tokens (Net::kv_cache)
 };
 struct BlockSpec {
   std::string pre;
@@ -74,6 +78,21 @@ struct Net {
   std::vector<void*> persistent;  // cudaMalloc'd for the life of the net
   std::unordered_map<std::string, Act*> debug_acts;
 
+  // ---- split forward (mdm_net_stage_io.stage)
+  int tape_stage = 0;          // stage (0 or 2) of the forward whose tape is held
+  Pool text_pool;              // workspace of the stage-1 passes, which run beside a held stage-0/2 tape
+  bool have_cond_io = false;   // a stage-1 forward with save_for_backward ran: its backward recomputes from cond_io
+  StepIO cond_io{};
+  // K/V cache of the cross-attention blocks (mdm_net_stage_io.cond_cache): block a's dense (batch * tokens, 2C) fp16 [k_c|v_c]
+  // starts at element a.kv_col * batch * tokens (kv_row = sum of 2C); valid for the (batch, tokens, level batches) it
+  // was filled with
+  long long kv_row = 0;
+  __half* kv_cache = nullptr;
+  size_t kv_cap = 0;           // elements allocated
+  uint64_t kv_epoch = 0;       // bumped on reallocation: graphs that read or write the cache record it
+  bool kv_valid = false;
+  int kv_key[2 + MDM_MAX_LEVELS] = {0, 0, 0, 0, 0, 0};
+
   // per-step state
   struct CondStep {
     int B = 0, S = 0, cd = 0;
@@ -93,6 +112,7 @@ struct Net {
     float* cemb = nullptr;  // (B, td)
     float* dcemb = nullptr;
     bool dcemb_init = false;
+    int kv_mode = 0;  // stage 2: mdm_net_stage_io.cond_cache
   } cs;
   struct LevelStep {
     float* temb = nullptr;      // (B, td) fp32
@@ -102,7 +122,7 @@ struct Net {
     bool dstemb_init = false;
   };
   std::deque<LevelStep> lsteps;
-  const mdm_net_io* io = nullptr;
+  const StepIO* io = nullptr;
   struct OutRec {
     float* nhwc = nullptr;  // [pix][out_ch]
     __half* d16 = nullptr;  // [pix][8] scaled gradient (filled by backward)
@@ -121,6 +141,7 @@ struct Net {
     for (auto& r : graphs) free_rec(r);
     if (cap_st != nullptr) cudaStreamDestroy(cap_st);
     for (void* p : persistent) cudaFree(p);
+    cudaFree(kv_cache);
   }
 
   // ---------------------------------------------------------------- parameters
@@ -367,6 +388,14 @@ struct Net {
     eng.d_amax = eng.d_scale + 2;
     persistent.push_back(eng.d_scale);
     eng.d_drop_seed = static_cast<unsigned long long*>(persist(sizeof(unsigned long long)));
+    for (auto& L : levels)
+      for (auto* blocks : {&L.down, &L.mid, &L.up})
+        for (auto& b : *blocks)
+          for (auto& a : b.attn)
+            if (a.cond) {
+              a.kv_col = kv_row;
+              kv_row += 2 * a.C;
+            }
   }
 
   // ---------------------------------------------------------------- weight packing
@@ -768,6 +797,7 @@ struct Net {
     __half* h16 = E.alloc<__half>(rows * C);
     __half *Pm = nullptr, *cn16 = nullptr, *kv = nullptr, *Pc = nullptr, *oself = nullptr;
     float *lnstats = nullptr, *astats = nullptr;
+    bool kv_cached = false;
     BOp Q{qkv, d, T, 3ll * C, 3 * nh, d, static_cast<long long>(T) * 3 * C, 0, false};
     if (cross) {
       // k_c, v_c = kv_cond(LayerNorm(cond))  (unet.py:304-305)
@@ -775,11 +805,15 @@ struct Net {
       Param &kw = P(a.pre + ".kv_cond.weight"), &kb = P(a.pre + ".kv_cond.bias");
       const long long crow = static_cast<long long>(B) * S;
       (void)lw; (void)lb; (void)kb;
-      kv = E.alloc<__half>(crow * 2 * C);
-      Epi e2;
-      e2.bias = a.kv_bias_fold;
-      e2.out_f16 = kv;
-      E.gemm_nt(cs.xhat16, cd, kw.w16, cd, static_cast<int>(crow), 2 * C, cd, e2);
+      // with the K/V cache on (stage 2, no tape) this block's slab of it: filled here (1) or read as it is (2)
+      kv_cached = cs.kv_mode != 0;
+      kv = kv_cached ? kv_cache + a.kv_col * cs.B * S : E.alloc<__half>(crow * 2 * C);
+      if (cs.kv_mode != 2) {
+        Epi e2;
+        e2.bias = a.kv_bias_fold;
+        e2.out_f16 = kv;
+        E.gemm_nt(cs.xhat16, cd, kw.w16, cd, static_cast<int>(crow), 2 * C, cd, e2);
+      }
     }
     if (fused) {
       if (E.training) {
@@ -870,7 +904,8 @@ struct Net {
     }
     if (!E.training) {
       E.rel(g1.y16); E.rel(g1.sums); E.rel(qkv); E.rel(Pm);
-      E.rel(h16); E.rel(cn16); E.rel(lnstats); E.rel(kv); E.rel(Pc);
+      E.rel(h16); E.rel(cn16); E.rel(lnstats); E.rel(Pc);
+      if (!kv_cached) E.rel(kv);
       E.rel(oself); E.rel(astats);
       if (a.ffn) {
         E.rel(g2.y16); E.rel(g2.sums); E.rel(u16); E.rel(gl16);
@@ -1260,8 +1295,9 @@ struct Net {
     E.rel(dh1);
   }
 
-  // forward_conditioning (unet.py:847-865) on the innermost level
-  void conditioning_fwd() {
+  // forward_conditioning (unet.py:847-865) on the innermost level. Stage 0 also runs the token LayerNorm of the
+  // cross-attention blocks (cond_norm_fwd), which belongs to forward_denoising; stage 1 stops at cond_emb.
+  void conditioning_fwd(int stage) {
     Engine& E = eng;
     const LevelSpec& L = levels.back();
     const int B = io->batch, S = io->tokens, td = L.c.temporal_dim;
@@ -1308,47 +1344,71 @@ struct Net {
       cs.cond32 = const_cast<float*>(io->lm);
     }
     for (int i = 0; i < cfg.num_lm_head_layers; ++i) lm_head_fwd(L.pre + "lm_head." + std::to_string(i), B, S);
-    {  // LayerNorm(cond) without its affine part, once per forward (31 blocks share it; unet.py:263,304)
-      cs.xhat16 = E.alloc<__half>(crow * cfg.cond_dim);
-      cs.lnstats = E.alloc<float>(crow * 2);
-      layernorm_fwd(cs.cond32, nullptr, nullptr, cs.xhat16, cs.lnstats, crow, cfg.cond_dim, E.st);
-    }
-    if (cfg.has_cond_emb) {
-      Param& cw = P(L.pre + "cond_emb.weight");
-      cs.y32 = E.alloc<float>(static_cast<long long>(B) * cfg.cond_dim);
-      cs.y16 = E.alloc<__half>(static_cast<long long>(B) * cfg.cond_dim);
-      masked_mean(cs.cond32, cs.mask, cs.y32, cs.y16, B, S, cfg.cond_dim, E.st);
-      cs.cemb = E.alloc<float>(static_cast<long long>(B) * td);
+    if (stage == 0) cond_norm_fwd();
+    if (!cfg.has_cond_emb) return;
+    Param& cw = P(L.pre + "cond_emb.weight");
+    cs.y32 = E.alloc<float>(static_cast<long long>(B) * cfg.cond_dim);
+    cs.y16 = E.alloc<__half>(static_cast<long long>(B) * cfg.cond_dim);
+    masked_mean(cs.cond32, cs.mask, cs.y32, cs.y16, B, S, cfg.cond_dim, E.st);
+    cs.cemb = E.alloc<float>(static_cast<long long>(B) * td);
+    {
       Epi e;
       e.out_f32 = cs.cemb;
       E.gemm_nt(cs.y16, cfg.cond_dim, cw.w16, cfg.cond_dim, B, td, cfg.cond_dim, e);
     }
     if (!E.training) return;
+    // replayed before the LayerNorm closure of stage 0: cs.dcond starts with the pooled-mean term
     E.tape.push_back([=]() {
+      if (cs.dcemb == nullptr) return;
       Engine& E = eng;
       const LevelSpec& L = levels.back();
       const long long crow = static_cast<long long>(B) * S;
-      if (cfg.has_cond_emb && cs.dcemb != nullptr) {
-        Param& cw = P(L.pre + "cond_emb.weight");
-        __half* d16 = E.alloc<__half>(static_cast<long long>(B) * td);
-        cast_colsum(cs.dcemb, d16, B, td, nullptr, nullptr, E.st);
-        float* dy = E.alloc<float>(static_cast<long long>(B) * cfg.cond_dim);
-        linear_bwd(d16, td, B, td, cfg.cond_dim, cs.y16, cfg.cond_dim, cw, nullptr, false, dy, 0);
-        if (cfg.has_lm_proj || cfg.num_lm_head_layers > 0) {
-          if (cs.dcond == nullptr) cs.dcond = E.alloc<float>(crow * cfg.cond_dim);
-          masked_mean_bwd(dy, cs.mask, cs.dcond, cs.dcond_init ? 1 : 0, B, S, cfg.cond_dim, E.st);
-          cs.dcond_init = true;
-        }
-        E.rel(d16);
-        E.rel(dy);
-      }
-      if (cs.dxhat_init) {
+      Param& cw = P(L.pre + "cond_emb.weight");
+      __half* d16 = E.alloc<__half>(static_cast<long long>(B) * td);
+      cast_colsum(cs.dcemb, d16, B, td, nullptr, nullptr, E.st);
+      float* dy = E.alloc<float>(static_cast<long long>(B) * cfg.cond_dim);
+      linear_bwd(d16, td, B, td, cfg.cond_dim, cs.y16, cfg.cond_dim, cw, nullptr, false, dy, 0);
+      if (cfg.has_lm_proj || cfg.num_lm_head_layers > 0) {
         if (cs.dcond == nullptr) cs.dcond = E.alloc<float>(crow * cfg.cond_dim);
-        layernorm_bwd(cs.cond32, nullptr, cs.lnstats, cs.dxhat, cs.dcond, cs.dcond_init ? 1 : 0, nullptr, nullptr, nullptr,
-                      crow, cfg.cond_dim, E.st);
+        masked_mean_bwd(dy, cs.mask, cs.dcond, cs.dcond_init ? 1 : 0, B, S, cfg.cond_dim, E.st);
         cs.dcond_init = true;
       }
+      E.rel(d16);
+      E.rel(dy);
     });
+  }
+
+  // LayerNorm(cond) without its affine part, once per forward: every cross-attention block folds its norm_cond affine
+  // into kv_cond and reads this (unet.py:263,304). Its closure adds the blocks' gradient to cs.dcond.
+  void cond_norm_fwd() {
+    Engine& E = eng;
+    const long long crow = static_cast<long long>(cs.B) * cs.S;
+    cs.xhat16 = E.alloc<__half>(crow * cfg.cond_dim);
+    cs.lnstats = E.alloc<float>(crow * 2);
+    layernorm_fwd(cs.cond32, nullptr, nullptr, cs.xhat16, cs.lnstats, crow, cfg.cond_dim, E.st);
+    if (!E.training) return;
+    E.tape.push_back([=]() {
+      if (!cs.dxhat_init) return;
+      Engine& E = eng;
+      if (cs.dcond == nullptr) cs.dcond = E.alloc<float>(crow * cfg.cond_dim);
+      layernorm_bwd(cs.cond32, nullptr, cs.lnstats, cs.dxhat, cs.dcond, cs.dcond_init ? 1 : 0, nullptr, nullptr, nullptr,
+                    crow, cfg.cond_dim, E.st);
+      cs.dcond_init = true;
+    });
+  }
+
+  // forward_denoising's side of the text (stage 2): the caller's tokens, pooled embedding and key mask
+  void cond_input_fwd() {
+    cs = CondStep();
+    cs.B = io->batch;
+    cs.S = io->tokens;
+    cs.cd = cfg.cond_dim;
+    cs.cross_mask = io->cross_mask;
+    cs.cemb = const_cast<float*>(io->cond_emb);
+    cs.kv_mode = io->cond_cache;
+    if (cfg.cond_dim <= 0) return;
+    cs.cond32 = const_cast<float*>(io->cond);
+    if (cs.kv_mode != 2) cond_norm_fwd();
   }
 
   // One SelfAttention1DBlock of lm_head (unet.py:316-446) on the fp32 token stream cs.cond32 (B*S rows of D):
@@ -1700,7 +1760,7 @@ struct Net {
   }
 
   // ---------------------------------------------------------------- entry points
-  void forward_body(const mdm_net_io* io_, cudaStream_t st) {
+  void forward_body(const StepIO* io_, cudaStream_t st) {
     eng.st = st;
     eng.training = io_->save_for_backward != 0;
     eng.tape.clear();
@@ -1718,14 +1778,18 @@ struct Net {
       MDM_CHECK(io->x_t[l] != nullptr && io->out[l] != nullptr, "missing x_t/out pointer");
       MDM_CHECK(io->res[l] % (1 << (cfg.levels[l].num_res - 1)) == 0, "resolution not divisible by the level's downsampling");
     }
-    if (cfg.cond_dim > 0) MDM_CHECK(io->lm != nullptr && io->tokens > 0, "conditioning required");
+    if (cfg.cond_dim > 0 && io->stage == 0) MDM_CHECK(io->lm != nullptr && io->tokens > 0, "conditioning required");
+    if (cfg.cond_dim > 0 && io->stage == 2)
+      MDM_CHECK(io->tokens > 0 && (io->cond != nullptr || io->cond_cache == 2), "stage 2 needs cond (batch, tokens, cond_dim)");
+    tape_stage = io->stage;
     {  // weight gradients on a side stream (engine.cuh); MDM_SIDE_WGRAD=0 keeps everything on one stream
       static const char* sw = getenv("MDM_SIDE_WGRAD");
       eng.side_enabled = sw != nullptr ? atoi(sw) != 0 : true;
       eng.ev_next = 0;
     }
     prepare_weights();
-    conditioning_fwd();
+    if (io->stage == 2) cond_input_fwd();
+    else conditioning_fwd(0);
     level_fwd(0, nullptr);
     have_tape = eng.training;
     io = nullptr;
@@ -1749,10 +1813,132 @@ struct Net {
       outs[l].d16 = eng.alloc<__half>(static_cast<long long>(B) * HW * 8);
       nchw_to_nhwc_f16(gio->dout[l], eng.d_scale, outs[l].d16, 8, B, cfg.out_channels, HW, st);
     }
-    replay_tape();
+    replay_tape(tape_stage == 0);
+    if (tape_stage == 2) {  // gradients of the caller's cond / cond_emb, unscaled
+      const long long n = static_cast<long long>(cs.B) * cs.S * cfg.cond_dim;
+      if (gio->dcond != nullptr && n > 0) {
+        if (cs.dcond_init) scale_f32(gio->dcond, cs.dcond, eng.d_inv_scale, n, st);
+        else MDM_CUDA(cudaMemsetAsync(gio->dcond, 0, sizeof(float) * n, st));
+      }
+      if (gio->dcond_emb != nullptr && cs.cemb != nullptr) {
+        const long long m = static_cast<long long>(cs.B) * levels.back().c.temporal_dim;
+        if (cs.dcemb != nullptr) scale_f32(gio->dcond_emb, cs.dcemb, eng.d_inv_scale, m, st);
+        else MDM_CUDA(cudaMemsetAsync(gio->dcond_emb, 0, sizeof(float) * m, st));
+      }
+    }
     eng.tape.clear();
     have_tape = false;
   }
+
+  // ---------------------------------------------------------------- stage 1: forward_conditioning alone
+  // Runs beside a held stage-0/2 tape (and any captured graph): on text_pool, with a tape of its own, and restores the
+  // held state when done. Its backward recomputes the text path from the recorded inputs and replays that tape at
+  // once, so the two stages' backwards can come in either order.
+  struct TextScope {
+    Net* n;
+    std::vector<std::function<void()>> tape;
+    CondStep cs;
+    const StepIO* io;
+    bool training;
+    TextScope(Net* net, bool train) : n(net), cs(net->cs), io(net->io), training(net->eng.training) {
+      tape.swap(n->eng.tape);
+      n->eng.training = train;
+      n->text_pool.reset();
+      n->eng.alt = &n->text_pool;
+    }
+    ~TextScope() {
+      n->eng.alt = nullptr;
+      n->eng.tape.swap(tape);
+      n->cs = cs;
+      n->io = io;
+      n->eng.training = training;
+    }
+  };
+
+  void stage1_forward(const StepIO* q, cudaStream_t st) {
+    MDM_CHECK(cfg.cond_dim > 0, "stage 1 needs a model with text conditioning (conditioning_feature_dim > 0)");
+    MDM_CHECK(q->batch > 0 && q->tokens > 0 && q->lm != nullptr && q->cond_out != nullptr,
+              "stage 1 needs batch, tokens, lm and cond_out");
+    MDM_CHECK(!cfg.has_cond_emb || q->cond_emb_out != nullptr, "stage 1 needs cond_emb_out: the model has cond_emb");
+    have_cond_io = false;
+    eng.st = st;
+    {
+      TextScope scope(this, false);
+      prepare_weights();
+      io = q;
+      conditioning_fwd(1);
+      const long long n = static_cast<long long>(q->batch) * q->tokens * cfg.cond_dim;
+      MDM_CUDA(cudaMemcpyAsync(q->cond_out, cs.cond32, sizeof(float) * n, cudaMemcpyDeviceToDevice, st));
+      if (cs.cemb != nullptr)
+        MDM_CUDA(cudaMemcpyAsync(q->cond_emb_out, cs.cemb,
+                                 sizeof(float) * q->batch * levels.back().c.temporal_dim, cudaMemcpyDeviceToDevice, st));
+    }
+    if (q->save_for_backward) {
+      cond_io = *q;
+      have_cond_io = true;
+    }
+  }
+
+  void stage1_backward(const mdm_net_grad_io* gio, cudaStream_t st) {
+    MDM_CHECK(have_cond_io, "a stage-1 backward needs a preceding stage-1 forward with save_for_backward=1");
+    have_cond_io = false;
+    eng.st = st;
+    TextScope scope(this, true);
+    prepare_weights();
+    io = &cond_io;
+    conditioning_fwd(1);
+    Engine& E = eng;
+    const long long n = static_cast<long long>(cs.B) * cs.S * cfg.cond_dim;
+    const long long m = static_cast<long long>(cs.B) * levels.back().c.temporal_dim;
+    // one gradient scale for both incoming gradients, derived as backward_body derives it from the output gradients
+    MDM_CUDA(cudaMemsetAsync(E.d_amax, 0, sizeof(float), st));
+    if (gio->dcond_in != nullptr) grad_amax(gio->dcond_in, n, E.d_amax, st);
+    if (gio->dcond_emb_in != nullptr && cs.cemb != nullptr) grad_amax(gio->dcond_emb_in, m, E.d_amax, st);
+    grad_scale_finalize(E.d_amax, E.d_scale, E.d_inv_scale, st);
+    cs.dcond = E.alloc<float>(n);
+    if (gio->dcond_in != nullptr) scale_f32(cs.dcond, gio->dcond_in, E.d_scale, n, st);
+    else MDM_CUDA(cudaMemsetAsync(cs.dcond, 0, sizeof(float) * n, st));
+    cs.dcond_init = true;
+    if (cs.cemb != nullptr) {
+      cs.dcemb = E.alloc<float>(m);
+      if (gio->dcond_emb_in != nullptr) scale_f32(cs.dcemb, gio->dcond_emb_in, E.d_scale, m, st);
+      else MDM_CUDA(cudaMemsetAsync(cs.dcemb, 0, sizeof(float) * m, st));
+    }
+    for (int i = static_cast<int>(E.tape.size()) - 1; i >= 0; --i) {
+      E.tape[i]();
+      E.side_join();
+    }
+  }
+
+  // ---------------------------------------------------------------- K/V cache (mdm_net_stage_io.cond_cache)
+  void kv_cache_begin(const StepIO* q) {
+    if (q->cond_cache == 0) return;
+    int key[2 + MDM_MAX_LEVELS] = {q->batch, q->tokens, 0, 0, 0, 0};
+    for (int l = 0; l < cfg.num_levels; ++l) key[2 + l] = level_batch_of(q, l);
+    if (q->cond_cache == 2) {
+      if (!kv_valid)
+        throw MdmFail("cond_cache 2: the K/V cache holds nothing valid (fill it with a cond_cache 1 forward; weight "
+                      "changes and rebinding parameters invalidate it)");
+      if (memcmp(key, kv_key, sizeof(key)) != 0)
+        throw MdmFail("cond_cache 2: the K/V cache was filled for batch " + std::to_string(kv_key[0]) + ", tokens " +
+                      std::to_string(kv_key[1]) + " (level batches " + std::to_string(kv_key[2]) + "..); this call has batch " +
+                      std::to_string(q->batch) + ", tokens " + std::to_string(q->tokens));
+      return;
+    }
+    kv_valid = false;
+    const size_t need = static_cast<size_t>(q->batch) * q->tokens * kv_row;
+    if (need > kv_cap) {
+      if (kv_cache != nullptr) MDM_CUDA(cudaDeviceSynchronize());  // replayed graphs may still read the old slot
+      cudaFree(kv_cache);
+      kv_cache = nullptr;
+      kv_cap = 0;
+      MDM_CUDA(cudaMalloc(&kv_cache, need * sizeof(__half)));
+      kv_cap = need;
+      ++kv_epoch;
+    }
+    memcpy(kv_key, key, sizeof(key));
+  }
+  static int level_batch_of(const mdm_net_io* q, int l) { return q->level_batch[l] > 0 ? q->level_batch[l] : q->batch; }
 
 
   // ---------------------------------------------------------------- CUDA graphs
@@ -1764,6 +1950,8 @@ struct Net {
   // (rebinding parameters, the pool returning memory to the driver) drops the recorded graphs.
   struct GraphRec {
     int training = 0, batch = 0, tokens = 0, has_mask = 0, has_micro = 0, apply_lm_mask = 0, dropout = 0;
+    int stage = 0, cond_cache = 0, has_cemb = 0;  // stage 2: the K/V cache mode and whether cond_emb is given
+    uint64_t kv_epoch = 0;
     int lb[MDM_MAX_LEVELS] = {0, 0, 0, 0}, res[MDM_MAX_LEVELS] = {0, 0, 0, 0};
     uint64_t bind_epoch = 0, pool_epoch = 0;
     float* x_t[MDM_MAX_LEVELS] = {nullptr, nullptr, nullptr, nullptr};
@@ -1771,8 +1959,10 @@ struct Net {
     float* dout[MDM_MAX_LEVELS] = {nullptr, nullptr, nullptr, nullptr};
     size_t x_bytes[MDM_MAX_LEVELS] = {0, 0, 0, 0};
     long long* times = nullptr;
-    float *lm = nullptr, *mask = nullptr, *micro = nullptr;
+    float *lm = nullptr, *mask = nullptr, *micro = nullptr;  // mask: lm_mask (stage 0) or cross_mask (stage 2)
     size_t lm_bytes = 0, mask_bytes = 0;
+    float *cond = nullptr, *cemb = nullptr, *dcond = nullptr, *dcemb = nullptr;  // stage 2
+    size_t cond_bytes = 0, cemb_bytes = 0;
     cudaGraphExec_t fwd = nullptr;
     // backward: one graph, or -- with a gradient-ready callback installed -- one graph per reported range, so the
     // caller's collective on range i is enqueued right after segment i and overlaps segments i+1..
@@ -1809,17 +1999,23 @@ struct Net {
     cudaFree(r.lm);
     cudaFree(r.mask);
     cudaFree(r.micro);
+    cudaFree(r.cond);
+    cudaFree(r.cemb);
+    cudaFree(r.dcond);
+    cudaFree(r.dcemb);
   }
-  bool same_key(const GraphRec& r, const mdm_net_io* q) const {
+  static const float* key_mask(const StepIO* q) { return q->stage == 2 ? q->cross_mask : q->lm_mask; }
+  bool same_key(const GraphRec& r, const StepIO* q) const {
     if (r.training != (q->save_for_backward != 0) || r.batch != q->batch || r.tokens != q->tokens ||
         r.apply_lm_mask != (q->apply_lm_mask != 0) || r.dropout != (q->dropout != 0) ||
-        r.has_mask != (q->lm_mask != nullptr) || r.has_micro != (q->micro_scale != nullptr))
+        r.has_mask != (key_mask(q) != nullptr) || r.has_micro != (q->micro_scale != nullptr) || r.stage != q->stage ||
+        r.cond_cache != q->cond_cache || r.has_cemb != (q->stage == 2 && q->cond_emb != nullptr))
       return false;
     for (int l = 0; l < cfg.num_levels; ++l)
       if (r.res[l] != q->res[l] || r.lb[l] != (q->level_batch[l] > 0 ? q->level_batch[l] : q->batch)) return false;
     return true;
   }
-  int find_rec(const mdm_net_io* q) {
+  int find_rec(const StepIO* q) {
     for (size_t i = 0; i < graphs.size(); ++i)
       if (same_key(graphs[i], q)) return static_cast<int>(i);
     if (graphs.size() >= 6) {  // bounded cache: evict the least recently used signature
@@ -1833,8 +2029,11 @@ struct Net {
     r.training = q->save_for_backward != 0;
     r.batch = q->batch;
     r.tokens = q->tokens;
-    r.has_mask = q->lm_mask != nullptr;
+    r.has_mask = key_mask(q) != nullptr;
     r.has_micro = q->micro_scale != nullptr;
+    r.stage = q->stage;
+    r.cond_cache = q->cond_cache;
+    r.has_cemb = q->stage == 2 && q->cond_emb != nullptr;
     r.apply_lm_mask = q->apply_lm_mask != 0;
     r.dropout = q->dropout != 0;
     for (int l = 0; l < cfg.num_levels; ++l) {
@@ -1846,9 +2045,19 @@ struct Net {
       if (r.training) MDM_CUDA(cudaMalloc(&r.dout[l], r.x_bytes[l] / cfg.in_channels * cfg.out_channels));
     }
     MDM_CUDA(cudaMalloc(&r.times, sizeof(long long) * r.batch));
-    if (q->lm != nullptr) {
+    if (q->stage == 0 && q->lm != nullptr) {
       r.lm_bytes = sizeof(float) * static_cast<size_t>(r.batch) * r.tokens * cfg.lm_dim;
       MDM_CUDA(cudaMalloc(&r.lm, r.lm_bytes));
+    }
+    if (q->stage == 2 && cfg.cond_dim > 0) {
+      r.cond_bytes = sizeof(float) * static_cast<size_t>(r.batch) * r.tokens * cfg.cond_dim;
+      if (q->cond_cache != 2) MDM_CUDA(cudaMalloc(&r.cond, r.cond_bytes));  // mode 2 does not read cond
+      if (r.training) MDM_CUDA(cudaMalloc(&r.dcond, r.cond_bytes));
+    }
+    if (r.has_cemb) {
+      r.cemb_bytes = sizeof(float) * static_cast<size_t>(r.batch) * levels.back().c.temporal_dim;
+      MDM_CUDA(cudaMalloc(&r.cemb, r.cemb_bytes));
+      if (r.training) MDM_CUDA(cudaMalloc(&r.dcemb, r.cemb_bytes));
     }
     if (r.has_mask) {
       r.mask_bytes = sizeof(float) * static_cast<size_t>(r.batch) * r.tokens;
@@ -1877,7 +2086,21 @@ struct Net {
     (void)cudaGetLastError();
   }
 
-  void forward(const mdm_net_io* io_, cudaStream_t st) {
+  void forward(const StepIO* io_, cudaStream_t st) {
+    if (io_->stage == 1) {  // eager: once per sampling run / training step, and it leaves any held tape alone
+      stage1_forward(io_, st);
+      return;
+    }
+    MDM_CHECK(io_->stage == 0 || io_->stage == 2, "mdm_net_stage_io.stage must be 0, 1 or 2");
+    MDM_CHECK(io_->cond_cache >= 0 && io_->cond_cache <= 2, "mdm_net_stage_io.cond_cache must be 0, 1 or 2");
+    MDM_CHECK(io_->cond_cache == 0 || (io_->stage == 2 && !io_->save_for_backward),
+              "cond_cache applies to stage-2 forwards without save_for_backward");
+    kv_cache_begin(io_);
+    forward_pass(io_, st);
+    if (io_->cond_cache == 1) kv_valid = true;
+  }
+
+  void forward_pass(const StepIO* io_, cudaStream_t st) {
     active_graph = -1;
     // on the caller's stream ahead of the eager, captured or replayed pass: the kernels read the seed from its slot
     if (io_->dropout) dropout_set_seed(eng.d_drop_seed, io_->dropout_seed, st);
@@ -1898,24 +2121,33 @@ struct Net {
       MDM_CUDA(cudaMemcpyAsync(r.x_t[l], io_->x_t[l], r.x_bytes[l], cudaMemcpyDeviceToDevice, st));
     MDM_CUDA(cudaMemcpyAsync(r.times, io_->times, sizeof(long long) * r.batch, cudaMemcpyDeviceToDevice, st));
     if (r.lm != nullptr) MDM_CUDA(cudaMemcpyAsync(r.lm, io_->lm, r.lm_bytes, cudaMemcpyDeviceToDevice, st));
-    if (r.has_mask) MDM_CUDA(cudaMemcpyAsync(r.mask, io_->lm_mask, r.mask_bytes, cudaMemcpyDeviceToDevice, st));
+    if (r.has_mask) MDM_CUDA(cudaMemcpyAsync(r.mask, key_mask(io_), r.mask_bytes, cudaMemcpyDeviceToDevice, st));
+    if (r.cond != nullptr) MDM_CUDA(cudaMemcpyAsync(r.cond, io_->cond, r.cond_bytes, cudaMemcpyDeviceToDevice, st));
+    if (r.cemb != nullptr) MDM_CUDA(cudaMemcpyAsync(r.cemb, io_->cond_emb, r.cemb_bytes, cudaMemcpyDeviceToDevice, st));
     if (r.has_micro)
       MDM_CUDA(cudaMemcpyAsync(r.micro, io_->micro_scale, sizeof(float) * r.batch, cudaMemcpyDeviceToDevice, st));
     eng.st = st;
     prepare_weights();  // outside the graph: only runs when the fp32 masters changed
     const bool valid = r.fwd != nullptr && r.bind_epoch == bind_epoch && r.pool_epoch == eng.pool.epoch() &&
+                       (r.cond_cache == 0 || r.kv_epoch == kv_epoch) &&
                        (!r.training || (!r.bwd.empty() && r.bwd_notifies == (ready_fn != nullptr)));
     if (!valid) {
       drop_graph(r);
       if (cap_st == nullptr) MDM_CUDA(cudaStreamCreateWithFlags(&cap_st, cudaStreamNonBlocking));
-      mdm_net_io sio = *io_;
+      StepIO sio = *io_;
       for (int l = 0; l < cfg.num_levels; ++l) {
         sio.x_t[l] = r.x_t[l];
         sio.out[l] = r.out[l];
       }
       sio.times = reinterpret_cast<const int64_t*>(r.times);
       sio.lm = r.lm;
-      sio.lm_mask = r.has_mask ? r.mask : nullptr;
+      if (r.stage == 2) {
+        sio.cond = r.cond;
+        sio.cond_emb = r.cemb;
+        sio.cross_mask = r.has_mask ? r.mask : nullptr;
+      } else {
+        sio.lm_mask = r.has_mask ? r.mask : nullptr;
+      }
       sio.micro_scale = r.has_micro ? r.micro : nullptr;
       const unsigned long long k0 = g_launch_count;
       MDM_CUDA(cudaStreamBeginCapture(cap_st, cudaStreamCaptureModeRelaxed));
@@ -1931,6 +2163,7 @@ struct Net {
       g_launch_count = k0;
       r.bind_epoch = bind_epoch;
       r.pool_epoch = eng.pool.epoch();
+      r.kv_epoch = kv_epoch;
       eng.st = st;
     }
     MDM_CUDA(cudaGraphLaunch(r.fwd, st));
@@ -1943,6 +2176,10 @@ struct Net {
   }
 
   void backward(const mdm_net_grad_io* gio, cudaStream_t st) {
+    if (gio->stage == 1) {
+      stage1_backward(gio, st);
+      return;
+    }
     if (active_graph < 0) {
       backward_body(gio, st);
       return;
@@ -1961,6 +2198,8 @@ struct Net {
       MDM_CHECK(have_tape, "graph mode: no recorded tape for this backward");
       mdm_net_grad_io sg{};
       for (int l = 0; l < cfg.num_levels; ++l) sg.dout[l] = (mask >> l) & 1 ? r.dout[l] : nullptr;
+      sg.dcond = r.dcond;
+      sg.dcond_emb = r.dcemb;
       const unsigned long long k0 = g_launch_count;
       MDM_CUDA(cudaStreamBeginCapture(cap_st, cudaStreamCaptureModeRelaxed));
       eng.capturing = true;  // weight gradients may fork onto the side stream (graph branches)
@@ -2004,11 +2243,17 @@ struct Net {
         ready_fn(ready_user, reinterpret_cast<void*>(r.bwd_ranges[i].first), reinterpret_cast<void*>(r.bwd_ranges[i].second));
     }
     g_launch_count += r.bwd_kernels;
+    if (gio->dcond != nullptr && r.dcond != nullptr)
+      MDM_CUDA(cudaMemcpyAsync(gio->dcond, r.dcond, r.cond_bytes, cudaMemcpyDeviceToDevice, st));
+    if (gio->dcond_emb != nullptr && r.dcemb != nullptr)
+      MDM_CUDA(cudaMemcpyAsync(gio->dcond_emb, r.dcemb, r.cemb_bytes, cudaMemcpyDeviceToDevice, st));
   }
 
   std::function<void(uintptr_t, uintptr_t)> seg_cut;  // set while a segmented backward is being captured
 
-  void replay_tape() {
+  // learn = false (a split backward): neither learns the closures' parameters nor reports ready ranges -- the text
+  // path's gradients are written by the other stage's backward, so no range is final here
+  void replay_tape(bool learn) {
     const int n = static_cast<int>(eng.tape.size());
     uintptr_t arena_lo = UINTPTR_MAX, arena_hi = 0;
     for (const Param& p : plist) {
@@ -2018,7 +2263,7 @@ struct Net {
       arena_hi = std::max(arena_hi, a + static_cast<uintptr_t>(p.numel) * sizeof(float));
     }
     // (while a backward is being captured the report cuts the graph into segments instead: see backward())
-    const bool notify = ready_fn != nullptr && static_cast<int>(learned.size()) == n && n > 0 && arena_hi > arena_lo;
+    const bool notify = learn && ready_fn != nullptr && static_cast<int>(learned.size()) == n && n > 0 && arena_hi > arena_lo;
     std::vector<uintptr_t> hi_prefix;  // highest gradient end address touched by closures 0..i
     if (notify) {
       hi_prefix.assign(n, arena_lo);
@@ -2043,7 +2288,7 @@ struct Net {
                 top ? (reinterpret_cast<uintptr_t>(top->g) - arena_lo) / 1048576.0 : 0.0, (arena_hi - arena_lo) / 1048576.0);
       }
     }
-    if (static_cast<int>(learned.size()) != n) learned.assign(n, {});
+    if (learn && static_cast<int>(learned.size()) != n) learned.assign(n, {});
     uintptr_t prev = arena_hi;
     final_lo = UINTPTR_MAX;
     struct Guard {
@@ -2059,6 +2304,7 @@ struct Net {
       cur_lookup.clear();
       eng.tape[i]();
       eng.side_join();  // weight-gradient work of this closure is ordered before anything later (and before a report)
+      if (!learn) continue;
       std::vector<int>& seen = learned[i];
       for (int idx : cur_lookup)
         if (std::find(seen.begin(), seen.end(), idx) == seen.end()) seen.push_back(idx);
@@ -2137,6 +2383,7 @@ int mdm_net_bind_param(mdm_net* net, const char* name, void* weight, void* grad)
     p.w = static_cast<float*>(weight);
     p.g = static_cast<float*>(grad);
     net->net.weights_dirty = true;
+    net->net.kv_valid = false;
   })
 }
 
@@ -2177,12 +2424,20 @@ int mdm_set_sm_reserve(int sms) {
 
 int mdm_net_weights_changed(mdm_net* net) {
   net->net.weights_dirty = true;
+  net->net.kv_valid = false;
   return 0;
 }
 
 int mdm_net_forward(mdm_net* net, const mdm_net_io* io, mdm_stream_t stream) {
+  return mdm_net_forward_stage(net, io, nullptr, stream);
+}
+
+int mdm_net_forward_stage(mdm_net* net, const mdm_net_io* io, const mdm_net_stage_io* stage, mdm_stream_t stream) {
   MDM_TRY({
-    net->net.forward(io, static_cast<cudaStream_t>(stream));
+    mdm::StepIO q{};
+    static_cast<mdm_net_io&>(q) = *io;
+    if (stage != nullptr) static_cast<mdm_net_stage_io&>(q) = *stage;
+    net->net.forward(&q, static_cast<cudaStream_t>(stream));
     MDM_CUDA(cudaGetLastError());
   })
 }
@@ -2198,6 +2453,14 @@ uint64_t mdm_net_workspace_bytes(const mdm_net* net) { return net->net.eng.pool.
 uint64_t mdm_net_workspace_high_water(const mdm_net* net) { return net->net.eng.pool.high_water(); }
 
 int64_t mdm_net_debug_fetch(mdm_net* net, const char* name, float* dst, int64_t max_elems, mdm_stream_t stream) {
+  const Net& N = net->net;
+  if (strcmp(name, "cond_kv") == 0) {  // the K/V cache as raw fp16 bits, two per float
+    if (!N.kv_valid) return -1;
+    const int64_t halves = static_cast<int64_t>(N.kv_key[0]) * N.kv_key[1] * N.kv_row, n = (halves + 1) / 2;
+    if (n > max_elems) return -2;
+    cudaMemcpyAsync(dst, N.kv_cache, sizeof(__half) * halves, cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream));
+    return n;
+  }
   auto it = net->net.debug_acts.find(name);
   if (it == net->net.debug_acts.end() || it->second->p == nullptr) return -1;
   const int64_t n = it->second->numel();

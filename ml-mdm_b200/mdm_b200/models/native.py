@@ -2,6 +2,7 @@
 include/mdm_b200.h).  torch is used for device memory, streams and autograd bookkeeping only."""
 import ctypes as C
 import os
+import weakref
 
 import torch
 
@@ -64,8 +65,28 @@ class NetIO(C.Structure):
     ]
 
 
+class StageIO(C.Structure):
+    """mdm_net_stage_io: which part of the denoiser mdm_net_forward_stage runs, and its text inputs / outputs."""
+    _fields_ = [
+        ("stage", C.c_int32),
+        ("cond_out", C.c_void_p),
+        ("cond_emb_out", C.c_void_p),
+        ("cond", C.c_void_p),
+        ("cond_emb", C.c_void_p),
+        ("cross_mask", C.c_void_p),
+        ("cond_cache", C.c_int32),
+    ]
+
+
 class NetGradIO(C.Structure):
-    _fields_ = [("dout", C.c_void_p * MAX_LEVELS)]
+    _fields_ = [
+        ("dout", C.c_void_p * MAX_LEVELS),
+        ("stage", C.c_int32),
+        ("dcond", C.c_void_p),
+        ("dcond_emb", C.c_void_p),
+        ("dcond_in", C.c_void_p),
+        ("dcond_emb_in", C.c_void_p),
+    ]
 
 
 def _ints(v, n=None):
@@ -143,6 +164,48 @@ class _DenoiseFn(torch.autograd.Function):
         return (None,) * 7 + (None,) * ctx.nlev + tuple(grads)
 
 
+class _ConditioningFn(torch.autograd.Function):
+    """forward_conditioning as one autograd node (mdm_net_io.stage = 1): lm_proj, the lm_head layers, the pooled mean
+    and cond_emb. Its backward (stage 1) recomputes the text path from the saved inputs and routes the gradients of
+    the text parameters only; the denoising node routes the others."""
+
+    @staticmethod
+    def forward(ctx, native, need_grad, apply_lm_mask, lm, mask, *text_params):
+        cond, cemb = native._conditioning(lm, mask, save=need_grad, apply_lm_mask=apply_lm_mask)
+        ctx.native = native
+        ctx.set_materialize_grads(False)
+        if not need_grad:
+            ctx.mark_non_differentiable(cond, cemb)
+        return cond, cemb
+
+    @staticmethod
+    def backward(ctx, dcond, dcemb):
+        native = ctx.native
+        grads = native._backward([], stage=1, dcond_in=dcond, dcemb_in=dcemb)
+        return (None,) * 5 + tuple(g for g, k in zip(grads, native.param_names) if k in native._text_names)
+
+
+class _DenoisingFn(torch.autograd.Function):
+    """forward_denoising as one autograd node (mdm_net_io.stage = 2), differentiable with respect to the tokens, the
+    pooled embedding and every parameter outside the text path."""
+
+    @staticmethod
+    def forward(ctx, native, nlev, need_grad, cache, times, cond, cond_emb, cross_mask, micro, *rest):
+        xs = rest[:nlev]
+        outs = native._forward(list(xs), times, None, None, micro, save=need_grad, stage=2, cond=cond,
+                               cond_emb=cond_emb, cross_mask=cross_mask, cache=cache)
+        ctx.native = native
+        ctx.nlev = nlev
+        ctx.want = (cond is not None and cond.requires_grad, cond_emb is not None and cond_emb.requires_grad)
+        ctx.set_materialize_grads(False)
+        return tuple(outs)
+
+    @staticmethod
+    def backward(ctx, *gouts):
+        grads, dcond, dcemb = ctx.native._backward(list(gouts), stage=2, want=ctx.want)
+        return (None,) * 5 + (dcond, dcemb, None, None) + (None,) * ctx.nlev + tuple(grads)
+
+
 ARENA_ALIGN = 64  # elements: every gradient view starts on a 256-byte boundary (vector loads in the optimiser sweep)
 
 
@@ -200,6 +263,15 @@ class NativeNet:
         # gradient-ready callback installed the backward is recorded as one graph per reported range.
         self.graphs = os.environ.get("MDM_NO_GRAPH") is None
         self.lib.mdm_net_set_graph_mode(self.handle, int(self.graphs))
+        # split forward: the text path's parameters (stage 1) and the state of the engine's K/V cache (stage 2)
+        inner = "inner_unet." * (self.cfg.num_levels - 1)
+        self._text_names = {k for k in self.names
+                            if k.startswith((inner + "lm_proj.", inner + "lm_head.", inner + "cond_emb."))}
+        self._text_clean = False  # the text parameters' arena slots are zero (a stage-2 backward just cleared it)
+        self.weights_epoch = 0    # bumped whenever the engine is told its weights changed or they are rebound
+        self._kv = None           # what the engine's K/V cache was filled from (see _cache_mode)
+        self._keep_text = None    # inputs of a stage-1 forward, kept for its backward
+        self._split_shapes = (None, None)
 
     def set_graph_mode(self, on):
         self.graphs = bool(on)
@@ -270,17 +342,77 @@ class NativeNet:
             self.params.append(p)
         self.sig = sig
         self.versions = None
+        self.weights_epoch += 1
 
     def _sync_weights(self):
         v = sum(p._version for p in self.params)
         if v != self.versions:
             self.lib.mdm_net_weights_changed(self.handle)
             self.versions = v
+            self.weights_epoch += 1
 
     # ---------------------------------------------------------------- public
     def run(self, xs, times, lm, mask, micros, apply_lm_mask=False):
         self._bind()
         self.apply_lm_mask = bool(apply_lm_mask)
+        micro = self._enter(micros)
+        # (Function.forward runs with grad mode off, so the decision is taken here)
+        need_grad = torch.is_grad_enabled() and any(p.requires_grad for p in self.params)
+        return _DenoiseFn.apply(self, len(xs), need_grad, times, lm, mask, micro, *xs, *self.params)
+
+    def run_conditioning(self, lm, mask, apply_lm_mask=False):
+        """forward_conditioning: (cond (B,S,cond_dim), cond_emb (B,temporal_dim) or None)."""
+        if self.cfg.cond_dim <= 0:
+            raise _lib.MdmError("forward_conditioning needs a model with text conditioning (conditioning_feature_dim > 0)")
+        if lm is None:
+            raise _lib.MdmError("forward_conditioning needs the conditioning tensor")
+        self._bind()
+        text = [p for p, k in zip(self.params, self.param_names) if k in self._text_names]
+        need_grad = torch.is_grad_enabled() and any(p.requires_grad for p in text)
+        cond, cemb = _ConditioningFn.apply(self, need_grad, bool(apply_lm_mask), lm, mask, *text)
+        return cond, (cemb if self.cfg.has_cond_emb else None)
+
+    def run_denoising(self, xs, times, cond_emb, cond, cross_mask, micros):
+        """forward_denoising on the engine (stage 2). Without autograd the K/V the cross-attention blocks compute from
+        `cond` are kept by the engine and reused while `cond`, `cross_mask` and the weights stay what they were."""
+        self._bind()
+        micro = self._enter(micros)
+        need_grad = torch.is_grad_enabled() and (any(p.requires_grad for p in self.params) or any(
+            t is not None and t.requires_grad for t in (cond, cond_emb)))
+        if self.cfg.cond_dim > 0 and cond is None:
+            raise _lib.MdmError("forward_denoising needs `conditioning` for a model with text conditioning")
+        cache = 0 if need_grad or self.cfg.cond_dim <= 0 else self._cache_mode(xs, cond, cross_mask)
+        outs = _DenoisingFn.apply(self, len(xs), need_grad, cache, times, cond, cond_emb, cross_mask, micro, *xs,
+                                  *self.params)
+        if cache == 1:
+            self._kv = self._kv_key(xs, cond, cross_mask)
+        return outs
+
+    def _kv_key(self, xs, cond, mask):
+        # identity (a weak reference: a freed tensor's address is reused) and in-place version of the tokens and mask,
+        # the weight state, and the shapes the cache was laid out for
+        def ident(t):
+            return None if t is None else (weakref.ref(t), t._version)
+        return (ident(cond), ident(mask), self.weights_epoch, tuple(x.shape[0] for x in xs), tuple(cond.shape))
+
+    def _cache_mode(self, xs, cond, mask):
+        """2 when the engine's K/V cache was filled from this very `cond` / `mask` (unchanged since) under the current
+        weights, else 1 (fill it)."""
+        self._sync_weights()  # an in-place weight update bumps weights_epoch here, before the comparison
+        old = self._kv
+        if old is None:
+            return 1
+        new = self._kv_key(xs, cond, mask)
+
+        def same(a, b):
+            if a is None or b is None:
+                return a is None and b is None
+            return a[0]() is not None and a[0]() is b[0]() and a[1] == b[1]
+        ok = same(old[0], new[0]) and same(old[1], new[1]) and old[2:] == new[2:]
+        return 2 if ok else 1
+
+    def _enter(self, micros):
+        """micro-conditioning tensor and the dropout (flag, seed) of the forward being entered."""
         micro = None
         if micros:
             micro = micros.get("scale", None)
@@ -293,11 +425,10 @@ class NativeNet:
             if training:
                 # from torch's default CPU generator: reproducible under torch.manual_seed, no device sync
                 self.dropout = (1, int(torch.randint(2**63 - 1, ())))
-        # (Function.forward runs with grad mode off, so the decision is taken here)
-        need_grad = torch.is_grad_enabled() and any(p.requires_grad for p in self.params)
-        return _DenoiseFn.apply(self, len(xs), need_grad, times, lm, mask, micro, *xs, *self.params)
+        return micro
 
-    def _forward(self, xs, times, lm, mask, micro, save, apply_lm_mask=False):
+    def _forward(self, xs, times, lm, mask, micro, save, apply_lm_mask=False, stage=0, cond=None, cond_emb=None,
+                 cross_mask=None, cache=0):
         self._sync_weights()
         if save and self.graphs and self.grad_arena is not None:
             lo, hi = self.grad_arena.data_ptr(), self.grad_arena.data_ptr() + self.grad_arena.numel() * 4
@@ -341,32 +472,99 @@ class NativeNet:
             if mask is not None:
                 mask = f32(mask)
                 io.lm_mask = mask.data_ptr()
+        sio = StageIO()
+        if stage == 2:
+            sio.stage = 2
+            sio.cond_cache = int(cache)
+            if cond is not None:
+                cond = f32(cond)
+                io.tokens = cond.shape[1]
+                sio.cond = cond.data_ptr()
+            if cond_emb is not None:
+                sio.cond_emb = f32(cond_emb).data_ptr()
+            if cross_mask is not None:
+                sio.cross_mask = f32(cross_mask).data_ptr()
         if micro is not None:
             micro = f32(micro)
             io.micro_scale = micro.data_ptr()
         io.save_for_backward = int(save)
+        if stage == 2 and save:
+            td = self.cfg.levels[self.cfg.num_levels - 1].temporal_dim
+            self._split_shapes = (tuple(cond.shape) if cond is not None else None, (B, td))
         io.apply_lm_mask = int(bool(apply_lm_mask))
         io.dropout, io.dropout_seed = self.dropout
         st = torch.cuda.current_stream().cuda_stream
-        _lib.check(self.lib.mdm_net_forward(self.handle, C.byref(io), C.c_void_p(st)), "mdm_net_forward")
+        if stage == 0:
+            _lib.check(self.lib.mdm_net_forward(self.handle, C.byref(io), C.c_void_p(st)), "mdm_net_forward")
+        else:
+            _lib.check(self.lib.mdm_net_forward_stage(self.handle, C.byref(io), C.byref(sio), C.c_void_p(st)),
+                       "mdm_net_forward_stage")
         self._keep = keep if save else None  # inputs must outlive the tape
         return outs
 
-    def _backward(self, gouts):
-        gio = NetGradIO()
+    def _conditioning(self, lm, mask, save, apply_lm_mask=False):
+        """mdm_net_forward with stage 1: (cond, cond_emb); cond_emb is an empty tensor for a model without one."""
+        self._sync_weights()
+        io = NetIO()
         keep = []
-        for i, g in enumerate(gouts):
-            if g is None:
-                continue
+
+        def f32(t):
+            t = t.detach()
+            if t.dtype != torch.float32 or not t.is_contiguous():
+                t = t.float().contiguous()
+            keep.append(t)
+            return t
+        lm = f32(lm)
+        if not lm.is_cuda:
+            raise _lib.MdmError("inputs must be CUDA tensors")
+        B, S = lm.shape[0], lm.shape[1]
+        sio = StageIO()
+        sio.stage = 1
+        io.batch, io.tokens = B, S
+        io.lm = lm.data_ptr()
+        if mask is not None:
+            io.lm_mask = f32(mask).data_ptr()
+        io.apply_lm_mask = int(bool(apply_lm_mask))
+        io.save_for_backward = int(save)
+        cond = torch.empty(B, S, self.cfg.cond_dim, device=lm.device, dtype=torch.float32)
+        td = self.cfg.levels[self.cfg.num_levels - 1].temporal_dim
+        cemb = torch.empty(B, td if self.cfg.has_cond_emb else 0, device=lm.device, dtype=torch.float32)
+        sio.cond_out = cond.data_ptr()
+        sio.cond_emb_out = cemb.data_ptr() if self.cfg.has_cond_emb else None
+        st = torch.cuda.current_stream().cuda_stream
+        _lib.check(self.lib.mdm_net_forward_stage(self.handle, C.byref(io), C.byref(sio), C.c_void_p(st)),
+                   "mdm_net_forward_stage (stage 1)")
+        self._keep_text = keep if save else None  # the stage-1 backward recomputes from these
+        return cond, cemb
+
+    def _backward(self, gouts, stage=0, dcond_in=None, dcemb_in=None, want=(False, False)):
+        """Stage 0: gradients of every parameter. Stage 1 (forward_conditioning): of the text parameters only, from the
+        incoming dcond_in / dcemb_in. Stage 2 (forward_denoising): of the other parameters, plus (d cond, d cond_emb)
+        where `want` asks for them. Parameters outside the stage get None."""
+        gio = NetGradIO()
+        gio.stage = stage
+        keep = []
+
+        def f32(g):
             g = g.detach()
             if g.dtype != torch.float32 or not g.is_contiguous():
                 g = g.float().contiguous()
             keep.append(g)
-            gio.dout[i] = g.data_ptr()
+            return g
+        for i, g in enumerate(gouts):
+            if g is None:
+                continue
+            gio.dout[i] = f32(g).data_ptr()
+        if stage == 1:
+            if dcond_in is not None:
+                gio.dcond_in = f32(dcond_in).data_ptr()
+            if dcemb_in is not None and dcemb_in.numel() > 0:
+                gio.dcond_emb_in = f32(dcemb_in).data_ptr()
+        mine = [stage == 0 or (k in self._text_names) == (stage == 1) for k in self.param_names]
         # fresh arena when existing .grad tensors alias the persistent one (gradient accumulation)
         arena = self.grad_arena
         lo, hi = arena.data_ptr(), arena.data_ptr() + arena.numel() * 4
-        aliased = any(p.grad is not None and lo <= p.grad.data_ptr() < hi for p in self.params)
+        aliased = any(p.grad is not None and lo <= p.grad.data_ptr() < hi for p, m in zip(self.params, mine) if m)
         if aliased:
             arena = torch.zeros_like(self.grad_arena)
             views = self._views(arena)
@@ -375,15 +573,36 @@ class NativeNet:
                                                        C.c_void_p(g.data_ptr()) if p.requires_grad else None), "bind")
             self.sig = None  # rebinding to the persistent arena happens at the next forward
         else:
-            if not self.arena_zeroed:  # the fused optimiser sweep (optim.FusedAdam) leaves it zeroed
+            views = self._views(arena)
+            if stage == 1:
+                # autograd runs the stage-2 backward first, which cleared the whole arena: zero only what is not clean
+                if not (self.arena_zeroed or self._text_clean):
+                    for v, m in zip(views, mine):
+                        if m:
+                            v.zero_()
+            elif not self.arena_zeroed:  # the fused optimiser sweep (optim.FusedAdam) leaves it zeroed
                 arena.zero_()
             self.arena_zeroed = False
-            views = self._views(arena)
+        self._text_clean = stage == 2
+        dcond = dcemb = None
+        if stage == 2:
+            if want[0]:
+                dcond = torch.empty(self._split_shapes[0], device=arena.device, dtype=torch.float32)
+                gio.dcond = dcond.data_ptr()
+            if want[1]:
+                dcemb = torch.empty(self._split_shapes[1], device=arena.device, dtype=torch.float32)
+                gio.dcond_emb = dcemb.data_ptr()
         st = torch.cuda.current_stream().cuda_stream
         self.active_arena = arena  # what a gradient-ready callback (parallel.GradientOverlap) indexes into
         _lib.check(self.lib.mdm_net_backward(self.handle, C.byref(gio), C.c_void_p(st)), "mdm_net_backward")
-        self._keep = None
-        return [g if p.requires_grad else None for p, g in zip(self.params, views)]
+        if stage == 1:
+            self._keep_text = None
+        else:
+            self._keep = None
+        grads = [g if (p.requires_grad and m) else None for p, g, m in zip(self.params, views, mine)]
+        if stage == 2:
+            return grads, dcond, dcemb
+        return grads
 
     def _views(self, arena):
         return arena_views(arena, self.params, self.offsets)

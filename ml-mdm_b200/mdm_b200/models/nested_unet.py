@@ -44,6 +44,11 @@ class NestedUNet(UNet):
     def model_type(self):
         return "nested_unet"
 
+    def forward_conditioning(self, conditioning, cond_mask):
+        """NestedUNet.forward_conditioning (nested_unet.py:165-166) hands the text to its innermost U-Net. The engine
+        runs the whole nest as one network, and its conditioning pass is the innermost level's text path."""
+        return super().forward_conditioning(conditioning, cond_mask)
+
     def _level_configs(self):
         return [self._config] + self.inner_unet._level_configs()
 

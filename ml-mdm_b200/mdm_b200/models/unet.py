@@ -281,3 +281,30 @@ class UNet(nn.Module):
         outs = self.native().run(xs, times, conditioning, cond_mask, micros,
                                  apply_lm_mask=bool(getattr(self, "fuse_lm_mask", False)))
         return outs[0] if single else list(outs)
+
+    def _require_top(self, what):
+        if bool(_cfg_get(self._config, "nesting", False)):
+            raise _lib.MdmError(f"{what}: this U-Net was built with nesting=True; the engine runs it as part of its "
+                                f"NestedUNet parent, so call {what} on the outermost NestedUNet")
+
+    def forward_conditioning(self, conditioning, cond_mask):
+        """UNet.forward_conditioning (unet.py:847-865): lm_proj, the lm_head layers, the pooled mean and cond_emb.
+        Returns (cond_emb, conditioning, cond_mask): cond_emb is None when the model has none, cond_mask is None unless
+        masked_cross_attention. Differentiable with respect to the text parameters."""
+        self._require_top("forward_conditioning")
+        native = self.native()
+        cond, cemb = native.run_conditioning(conditioning, cond_mask,
+                                             apply_lm_mask=bool(getattr(self, "fuse_lm_mask", False)))
+        return cemb, cond, (cond_mask if native.cfg.masked_cross_attention else None)
+
+    def forward_denoising(self, x_t, times, cond_emb=None, conditioning=None, cond_mask=None, micros={}):
+        """UNet.forward_denoising (unet.py:935-969) / NestedUNet.forward_denoising (nested_unet.py:168-230): the
+        denoiser on given text features. x_t is a tensor for a UNet, a list (high -> low resolution) for a NestedUNet.
+        Differentiable with respect to conditioning, cond_emb and the parameters outside the text path. Without
+        autograd, the K/V the cross-attention blocks compute from `conditioning` are kept by the engine and reused by
+        the next call with the same (unmodified) conditioning / cond_mask tensors under unchanged weights."""
+        self._require_top("forward_denoising")
+        single = not isinstance(x_t, (list, tuple))
+        xs = [x_t] if single else list(x_t)
+        outs = self.native().run_denoising(xs, times, cond_emb, conditioning, cond_mask, micros)
+        return outs[0] if single else list(outs)

@@ -73,6 +73,7 @@ class Sampler(nn.Module):
         if self._config.loss_target_type is None:
             self._config.loss_target_type = self._config.prediction_type
         self._level_tables = {}
+        self._text = None  # (lm_outputs, lm_mask, forward_conditioning of them) during a sampling run
 
     # ---- schedule (samplers.py:201-231,255-264)
     def get_noise_schedule(self, schedule_type, n_steps: int, sampler_config):
@@ -229,13 +230,44 @@ class Sampler(nn.Module):
         """Classifier-free guidance wrapper (samplers.py:435-459): rows are [uncond; cond]."""
         if guidance_scale != 1:
             assert x_t.shape[0] * 2 == lm_outputs.shape[0]
-            pred, extras = model(torch.cat([x_t] * 2), torch.cat([t, t]), lm_outputs, lm_mask, micros=micros)
+            pred, extras = self._model(model, torch.cat([x_t] * 2), torch.cat([t, t]), lm_outputs, lm_mask, micros)
             u, c = pred.chunk(2)
             pred = self._cfg(u, c, guidance_scale)
             extras = extras.chunk(2)[1]
         else:
-            pred, extras = model(x_t, t, lm_outputs, lm_mask, micros)
+            pred, extras = self._model(model, x_t, t, lm_outputs, lm_mask, micros)
         return pred, extras
+
+    # ---- text encoded once per sampling run
+    def _encode_text(self, model, lm_outputs, lm_mask):
+        """forward_conditioning of the whole run, when `model` is this package's Model / NestedModel (a subclass that
+        overrides forward, or any other wrapper, is called as it is at every step). The steps then evaluate
+        forward_denoising on it, and the engine reuses the cross-attention K/V it computed at the first step."""
+        from .diffusion import Model, NestedModel
+        from .models import UNet
+
+        if lm_outputs is None or getattr(type(model), "forward", None) not in (Model.forward, NestedModel.forward):
+            return None
+        if isinstance(model, NestedModel) and not getattr(model.diffusion_config, "no_use_residual", False):
+            return None  # NestedModel.forward raises for the residual mode; let it
+        vm = model.vision_model
+        if not isinstance(vm, UNet) or vm.native().cfg.cond_dim <= 0:
+            return None
+        return lm_outputs, lm_mask, vm.forward_conditioning(lm_outputs, lm_mask)
+
+    def _model(self, model, x_t, t, lm_outputs, lm_mask, micros):
+        """model(x_t, t, lm_outputs, lm_mask, micros), through the run's encoded text when there is one for exactly
+        these lm_outputs / lm_mask tensors."""
+        enc = getattr(self, "_text", None)
+        if enc is None or enc[0] is not lm_outputs or enc[1] is not lm_mask:
+            return model(x_t, t, lm_outputs, lm_mask, micros)
+        from .diffusion import NestedModel
+
+        cond_emb, cond, cmask = enc[2]
+        out = model.vision_model.forward_denoising(x_t, t, cond_emb, cond, cmask, micros)
+        if isinstance(model, NestedModel):
+            return out
+        return out, out.new_ones(()).expand_as(out)  # Model.forward's (outputs, variances placeholder)
 
     @staticmethod
     def _cfg(u, c, w):
@@ -294,16 +326,20 @@ class Sampler(nn.Module):
         seq = [x_t] if return_sequence else []
         x0, extra = None, None
         with torch.no_grad():
-            for i, tt in enumerate(timesteps[:-1]):
-                t_last = timesteps[i + 1] if resample_steps else None
-                x0, x_t, extra = self.get_xt_minus_1(model, int(tt), x_t, lm_outputs, lm_mask, micros,
-                                                     time_step_last=None if t_last is None else int(t_last),
-                                                     guidance_scale=guidance_scale, ddim_eta=ddim_eta,
-                                                     return_details=True)
-                if yield_output:
-                    yield self._postprocess(x_t, x0, extra, **post_args)
-                if return_sequence:
-                    seq.append(self._postprocess(x_t))
+            self._text = self._encode_text(model, lm_outputs, lm_mask)
+            try:
+                for i, tt in enumerate(timesteps[:-1]):
+                    t_last = timesteps[i + 1] if resample_steps else None
+                    x0, x_t, extra = self.get_xt_minus_1(model, int(tt), x_t, lm_outputs, lm_mask, micros,
+                                                         time_step_last=None if t_last is None else int(t_last),
+                                                         guidance_scale=guidance_scale, ddim_eta=ddim_eta,
+                                                         return_details=True)
+                    if yield_output:
+                        yield self._postprocess(x_t, x0, extra, **post_args)
+                    if return_sequence:
+                        seq.append(self._postprocess(x_t))
+            finally:
+                self._text = None
             if return_sequence:
                 seq[-1] = self._scale_clip(seq[-1], 1.0, True)
                 yield seq
@@ -399,6 +435,6 @@ class NestedSampler(Sampler):
         """samplers.py:774-793."""
         if guidance_scale != 1:
             assert x_t[0].shape[0] * 2 == lm_outputs.shape[0]
-            p_t = model([torch.cat([x] * 2) for x in x_t], torch.cat([t] * 2), lm_outputs, lm_mask, micros)
+            p_t = self._model(model, [torch.cat([x] * 2) for x in x_t], torch.cat([t] * 2), lm_outputs, lm_mask, micros)
             return [self._cfg(*p.chunk(2), guidance_scale) for p in p_t]
-        return model(x_t, t, lm_outputs, lm_mask, micros)
+        return self._model(model, x_t, t, lm_outputs, lm_mask, micros)
