@@ -121,7 +121,7 @@ typedef struct mdm_level_cfg {
   int32_t skip_mid_blocks;
   int32_t nesting;            /* this U-Net sits inside another one (UNetConfig.nesting) */
   int32_t skip_normalization; /* NestedUNetConfig.skip_normalization (outer levels only) */
-  int32_t has_micro_scale;    /* micro_conditioning == "scale:<default>" */
+  int32_t has_micro_scale;    /* micro_conditioning == "scale:<default>" (mdm_net_create; other strings: mdm_micro_cfg) */
   float micro_scale_default;
   /* ResNetConfig.dropout in [0, 1]: nn.Dropout between SiLU(norm2) and conv2 of every ResNet of this level
    * (unet.py:208,233-235), applied when mdm_net_io.dropout is 1 */
@@ -166,7 +166,7 @@ typedef struct mdm_net_io {
   const int64_t* times;             /* (batch,) */
   const float* lm;                  /* (batch, tokens, lm_dim) fp32 */
   const float* lm_mask;             /* (batch, tokens) fp32 0/1, or NULL */
-  const float* micro_scale;         /* (batch,) fp32 or NULL => per-level default (unet.py:924) */
+  const float* micro_scale;         /* (batch,) fp32 or NULL => per-level default (unet.py:924): the key "scale" */
   float* out[MDM_MAX_LEVELS];       /* NCHW fp32 predictions, same shapes as x_t */
   int32_t save_for_backward;
   /* Mixed-resolution batches (NestedDiffusionConfig.mixed_ratio, diffusion.py:262-274; nested_unet.py:180,
@@ -188,7 +188,8 @@ typedef struct mdm_net_io {
 } mdm_net_io;
 
 /* CUDA-graph execution of forward / backward (off by default). With it on, the first call with a given shape
- * signature (batch, per-level batch, resolutions, tokens, mask/micro presence, save_for_backward, dropout, stage,
+ * signature (batch, per-level batch, resolutions, tokens, mask presence, which micro keys have values,
+ * save_for_backward, dropout, stage,
  * cond_cache, cond_emb presence; stage-1 calls always run eagerly) runs
  * eagerly, the
  * second is captured and later ones replay the captured graphs: inputs / output gradients are copied into static
@@ -233,6 +234,40 @@ typedef struct mdm_net_stage_io {
   int32_t cond_cache;
 } mdm_net_stage_io;
 int mdm_net_forward_stage(mdm_net* net, const mdm_net_io* io, const mdm_net_stage_io* stage, mdm_stream_t stream);
+
+/* ---- general micro-conditioning (UNetConfig.micro_conditioning = "LABEL:DEFAULT,LABEL:DEFAULT,...", unet.py:615-629,
+ * 920-933). Each level of the nest has its own keys, order and defaults. Per key, in the level's order, the level owns
+ * cond_layers.<key>.0 = Linear(td/4, td) and cond_layers.<key>.1 = Linear(td, td), and adds
+ *   layer1(silu(layer0(sincos(m * t_emb))))   with m = clamp(v / default, max=1) * default for the key "scale",
+ *                                             and m = v * 1000 for every other key
+ * to its temb, v being the key's value of the sample or, when absent, the level's default. mdm_net_create is
+ * mdm_net_create_micro with the table {"scale": micro_scale_default} at every level that sets has_micro_scale, and the
+ * old forward entry points pass mdm_net_io.micro_scale as the value of the key "scale". Unlike the reference, a "scale"
+ * default of 0 (0/0 there) is refused. */
+#define MDM_MAX_MICRO 8       /* distinct keys of a nest */
+#define MDM_MICRO_NAME_LEN 32 /* bytes of a key name, the terminating NUL included */
+
+typedef struct mdm_micro_cfg {
+  int32_t num_keys;                              /* distinct keys of the nest: first appearance, outermost level first */
+  char names[MDM_MAX_MICRO][MDM_MICRO_NAME_LEN]; /* NUL-terminated, non-empty, distinct */
+  int32_t level_num_keys[MDM_MAX_LEVELS];
+  int32_t level_keys[MDM_MAX_LEVELS][MDM_MAX_MICRO];   /* indices into names, in the level's order, no repeats */
+  float level_defaults[MDM_MAX_LEVELS][MDM_MAX_MICRO]; /* the level's default of each of its keys */
+} mdm_micro_cfg;
+
+/* cfg must not set has_micro_scale at any level: the table says everything about micro-conditioning. */
+int mdm_net_create_micro(const mdm_net_cfg* cfg, const mdm_micro_cfg* micro, mdm_net** out);
+
+typedef struct mdm_net_micro_io {
+  /* values[k]: (batch,) fp32 values of the table's key k, or NULL => each level's default. Level l reads the leading
+   * level_batch[l] rows. */
+  const float* values[MDM_MAX_MICRO];
+} mdm_net_micro_io;
+
+/* mdm_net_forward_stage (stage NULL: mdm_net_forward) with the values of the micro table's keys (micro NULL: every key
+ * takes its default). io->micro_scale must be NULL. Stage-1 forwards read no micro values. */
+int mdm_net_forward_micro(mdm_net* net, const mdm_net_io* io, const mdm_net_stage_io* stage,
+                          const mdm_net_micro_io* micro, mdm_stream_t stream);
 
 typedef struct mdm_net_grad_io {
   const float* dout[MDM_MAX_LEVELS]; /* d loss / d out[l], NCHW fp32; NULL => zero */

@@ -1448,21 +1448,26 @@ __global__ void unfold_ln_grads_kernel(const float* __restrict__ dWf, const floa
 }
 
 // ------------------------------------------------------------------ embeddings / activations
-__global__ void sinusoid_embed_kernel(const long long* __restrict__ times, const float* __restrict__ values,
-                                      float const_value, float clamp_default, const float* __restrict__ freq,
-                                      int B, int half, __half* __restrict__ e16) {
+// grid.y: the key (1 for the time embedding). sinf/cosf, not the fast intrinsics: micro arguments reach ~1e3 rad.
+__global__ void sinusoid_embed_kernel(const long long* __restrict__ times, MicroKeys micro,
+                                      const float* __restrict__ freq, int B, int half, long long key_stride,
+                                      __half* __restrict__ e16) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= B * half) return;
-  const int b = idx / half, i = idx - b * half;
+  const int b = idx / half, i = idx - b * half, k = blockIdx.y;
   float v;
-  if (times != nullptr) v = static_cast<float>(times[b]);
-  else if (values != nullptr) v = values[b];
-  else v = const_value;
-  if (clamp_default > 0.f) v = fminf(v / clamp_default, 1.0f) * clamp_default;
+  if (times != nullptr) {
+    v = static_cast<float>(times[b]);
+  } else {
+    const float d = micro.defaults[k];
+    v = micro.values[k] != nullptr ? micro.values[k][b] : d;
+    v = (micro.scale_mask >> k) & 1u ? fminf(v / d, 1.0f) * d : v * 1000.0f;
+  }
   const float w = freq[i];
   const float a = v * w;
-  e16[static_cast<long long>(b) * 2 * half + i] = __float2half_rn(sinf(a));
-  e16[static_cast<long long>(b) * 2 * half + half + i] = __float2half_rn(cosf(a));
+  __half* e = e16 + k * key_stride + static_cast<long long>(b) * 2 * half;
+  e[i] = __float2half_rn(sinf(a));
+  e[half + i] = __float2half_rn(cosf(a));
 }
 
 __global__ void silu_f16_kernel(const float* __restrict__ x, __half* __restrict__ y, long long n) {
@@ -2099,10 +2104,13 @@ void unfold_ln_grads(const float* dWf, const float* dbf, const float* W, const f
   MDM_LAUNCHED();
 }
 
-void sinusoid_embed(const long long* times, const float* values, float const_value, float clamp_default,
-                    const float* freq, int B, int half, __half* e16, cudaStream_t st) {
-  sinusoid_embed_kernel<<<static_cast<unsigned>(cdiv(static_cast<long long>(B) * half, 256)), 256, 0, st>>>(
-      times, values, const_value, clamp_default, freq, B, half, e16);
+void sinusoid_embed(const long long* times, const MicroKeys* micro, const float* freq, int B, int half,
+                    long long key_stride, __half* e16, cudaStream_t st) {
+  MicroKeys keys{};
+  if (micro != nullptr) keys = *micro;
+  const dim3 grid(static_cast<unsigned>(cdiv(static_cast<long long>(B) * half, 256)),
+                  times != nullptr ? 1u : static_cast<unsigned>(keys.num));
+  sinusoid_embed_kernel<<<grid, 256, 0, st>>>(times, keys, freq, B, half, key_stride, e16);
   MDM_LAUNCHED();
 }
 void silu_f16(const float* x, __half* y16, long long n, cudaStream_t st) {

@@ -107,12 +107,20 @@ void unfold_ln_grads(const float* dWf, const float* dbf, const float* W, const f
                      float* dw, float* db, int rows, int D, cudaStream_t st);
 
 // ---- embeddings / small elementwise
+// The micro-conditioning keys of one level, in its order (unet.py:920-933).
+constexpr int kMaxMicroKeys = 8;  // MDM_MAX_MICRO
+struct MicroKeys {
+  int num;
+  const float* values[kMaxMicroKeys];  // (B,) fp32, or null: the key takes its default
+  float defaults[kMaxMicroKeys];
+  unsigned scale_mask;  // bit k: key k is "scale" (clamp(v/default, max=1)*default); otherwise v*1000
+};
 // e16[b][0:half]=sin(v*w_i), [half:2half]=cos(v*w_i); w = the reference's t_emb buffer
 // exp(-ln(1e4) i/half) (unet.py:600-603,834-836), bound from the host so it is bit-identical.
-// times (int64) or values (fp32) -- exactly one non-null. clamp_default > 0 applies the micro
-// "scale" transform clamp(v/default, max=1)*default (unet.py:924-929).
-void sinusoid_embed(const long long* times, const float* values, float const_value, float clamp_default,
-                    const float* freq, int B, int half, __half* e16, cudaStream_t st);
+// Exactly one of times / micro is non-null. times (int64): one embedding, v = times[b]. micro: one embedding per key
+// k, at e16 + k * key_stride, of v = the key's transform of its value (unet.py:924-929).
+void sinusoid_embed(const long long* times, const MicroKeys* micro, const float* freq, int B, int half,
+                    long long key_stride, __half* e16, cudaStream_t st);
 void silu_f16(const float* x, __half* y16, long long n, cudaStream_t st);
 // dx (=|+=) dy * silu'(x)
 void silu_bwd(const float* x, const float* dy, float* dx, long long n, int acc, cudaStream_t st);

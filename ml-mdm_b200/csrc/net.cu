@@ -26,8 +26,10 @@ namespace mdm {
 
 unsigned long long g_graph_launches = 0;
 
-// what one forward call is given: the io and the split-forward fields beside it (mdm_net_forward_stage)
-struct StepIO : mdm_net_io, mdm_net_stage_io {};
+// what one forward call is given: the io, the split-forward fields beside it (mdm_net_forward_stage) and the values of
+// the micro-conditioning keys (mdm_net_forward_micro; mdm_net_io.micro_scale is moved to the key "scale" on entry)
+struct StepIO : mdm_net_io, mdm_net_stage_io, mdm_net_micro_io {};
+static_assert(kMaxMicroKeys == MDM_MAX_MICRO, "MicroKeys holds one level's keys");
 
 namespace {
 
@@ -57,6 +59,11 @@ struct LevelSpec {
   int film_total = 0;
   int feat_ch = 0;
   bool innermost = false;
+  // micro-conditioning keys in the level's order: "<pre>cond_layers.<key>", the key's index in the net's table
+  // (mdm_net_micro_io.values) and its default / transform (values are bound per step)
+  std::vector<std::string> micro_pre;
+  std::vector<int> micro_slot;
+  MicroKeys micro{};
   // persistent packed time-layer operands
   __half* tl_w16 = nullptr;  // [film_total][td]
   float* tl_bias = nullptr;  // [film_total]
@@ -68,6 +75,8 @@ int round8(int x) { return (x + 7) / 8 * 8; }
 
 struct Net {
   mdm_net_cfg cfg;
+  mdm_micro_cfg micro{};  // the nest's micro-conditioning table (mdm_net_create_micro)
+  int scale_slot = -1;    // index of the key "scale" in it, -1 if absent: where mdm_net_io.micro_scale goes
   std::vector<LevelSpec> levels;
   std::vector<Param> plist;
   std::unordered_map<std::string, int> pindex;
@@ -255,8 +264,36 @@ struct Net {
   }
 
   // Mirrors the bookkeeping of UNet.__init__ (unet.py:631-747): channel/skip arithmetic only.
+  // the micro table of mdm_net_create_micro: well-formed names, per-level keys and defaults
+  void check_micro() {
+    MDM_CHECK(micro.num_keys >= 0 && micro.num_keys <= MDM_MAX_MICRO, "mdm_micro_cfg.num_keys must lie in [0, MDM_MAX_MICRO]");
+    for (int k = 0; k < micro.num_keys; ++k) {
+      const char* nm = micro.names[k];
+      MDM_CHECK(memchr(nm, 0, MDM_MICRO_NAME_LEN) != nullptr && nm[0] != 0,
+                "micro-conditioning key names must be non-empty and shorter than MDM_MICRO_NAME_LEN");
+      for (int j = 0; j < k; ++j)
+        if (strcmp(nm, micro.names[j]) == 0) throw MdmFail(std::string("micro-conditioning key '") + nm + "' is listed twice");
+      if (strcmp(nm, "scale") == 0) scale_slot = k;
+    }
+    for (int li = 0; li < cfg.num_levels; ++li) {
+      const int n = micro.level_num_keys[li];
+      MDM_CHECK(n >= 0 && n <= micro.num_keys, "mdm_micro_cfg.level_num_keys must lie in [0, num_keys]");
+      for (int j = 0; j < n; ++j) {
+        const int k = micro.level_keys[li][j];
+        MDM_CHECK(k >= 0 && k < micro.num_keys, "mdm_micro_cfg.level_keys must index the table");
+        for (int i = 0; i < j; ++i) MDM_CHECK(micro.level_keys[li][i] != k, "a level lists a micro-conditioning key twice");
+        const float d = micro.level_defaults[li][j];
+        if (!isfinite(d)) throw MdmFail(std::string("micro-conditioning key '") + micro.names[k] + "' has a non-finite default");
+        // the reference divides by the default of "scale" (unet.py:926): 0 would give 0/0
+        if (k == scale_slot && d == 0.f)
+          throw MdmFail("micro-conditioning key 'scale' needs a non-zero default (clamp(v / default, max=1) * default)");
+      }
+    }
+  }
+
   void build() {
     MDM_CHECK(cfg.num_levels >= 1 && cfg.num_levels <= MDM_MAX_LEVELS, "bad num_levels");
+    check_micro();
     MDM_CHECK(cfg.in_channels * 9 <= 32, "conv_in packs 9*Cin into one 32-wide k block");
     std::string pre;
     for (int li = 0; li < cfg.num_levels; ++li) {
@@ -278,11 +315,19 @@ struct Net {
       add_param(pre + "temb_layer2.weight", {td, td}, 1);
       add_param(pre + "temb_layer2.bias", {td}, 0);
       if (L.innermost && cfg.has_cond_emb) add_param(pre + "cond_emb.weight", {td, cfg.cond_dim}, 1);
-      if (c.has_micro_scale) {
-        add_param(pre + "cond_layers.scale.0.weight", {td, td / 4}, 1);
-        add_param(pre + "cond_layers.scale.0.bias", {td}, 0);
-        add_param(pre + "cond_layers.scale.1.weight", {td, td}, 1);
-        add_param(pre + "cond_layers.scale.1.bias", {td}, 0);
+      MDM_CHECK(!c.has_micro_scale, "has_micro_scale is for mdm_net_create; with mdm_net_create_micro the table says it");
+      L.micro.num = micro.level_num_keys[li];
+      for (int j = 0; j < L.micro.num; ++j) {
+        const int k = micro.level_keys[li][j];
+        const std::string cl = pre + "cond_layers." + micro.names[k];
+        add_param(cl + ".0.weight", {td, td / 4}, 1);
+        add_param(cl + ".0.bias", {td}, 0);
+        add_param(cl + ".1.weight", {td, td}, 1);
+        add_param(cl + ".1.bias", {td}, 0);
+        L.micro_pre.push_back(cl);
+        L.micro_slot.push_back(k);
+        L.micro.defaults[j] = micro.level_defaults[li][j];
+        if (strcmp(micro.names[k], "scale") == 0) L.micro.scale_mask |= 1u << j;
       }
       add_param(pre + "conv_in.weight", {c.channels[0], cfg.in_channels, 3, 3}, 3);
       add_param(pre + "conv_in.bias", {c.channels[0]}, 0);
@@ -1537,17 +1582,30 @@ struct Net {
     const long long n = static_cast<long long>(B) * td;
     __half* e16 = E.alloc<__half>(static_cast<long long>(B) * (td / 4));
     const float* freq = P(L.pre + "t_emb").w;
-    sinusoid_embed(reinterpret_cast<const long long*>(io->times), nullptr, 0.f, 0.f, freq, B, half, e16, E.st);
-    MlpRec trec{}, mrec{};
+    sinusoid_embed(reinterpret_cast<const long long*>(io->times), nullptr, freq, B, half, 0, e16, E.st);
+    MlpRec trec{};
     float* t = embed_mlp_fwd(L.pre + "temb_layer1", L.pre + "temb_layer2", e16, B, td, &trec);
     ls->temb = t;
     if (cs.cemb != nullptr) add_f32(t, t, cs.cemb, n, E.st);
-    const bool micro = L.c.has_micro_scale != 0;
-    if (micro) {
-      __half* m16 = E.alloc<__half>(static_cast<long long>(B) * (td / 4));
-      sinusoid_embed(nullptr, io->micro_scale, L.c.micro_scale_default, L.c.micro_scale_default, freq, B, half, m16,
-                     E.st);
-      float* m = embed_mlp_fwd(L.pre + "cond_layers.scale.0", L.pre + "cond_layers.scale.1", m16, B, td, &mrec);
+    // micro-conditioning (unet.py:920-933): the keys' terms are summed in the level's order, then added to temb
+    const int nkeys = L.micro.num;
+    std::vector<MlpRec> mrec(nkeys);
+    if (nkeys > 0) {
+      MicroKeys keys = L.micro;
+      for (int j = 0; j < nkeys; ++j) keys.values[j] = io->values[L.micro_slot[j]];
+      const long long stride = (static_cast<long long>(B) * (td / 4) + 127) / 128 * 128;  // 256-byte aligned operands
+      __half* m16 = E.alloc<__half>(stride * nkeys);
+      sinusoid_embed(nullptr, &keys, freq, B, half, stride, m16, E.st);
+      float* m = nullptr;
+      for (int j = 0; j < nkeys; ++j) {
+        float* mj = embed_mlp_fwd(L.micro_pre[j] + ".0", L.micro_pre[j] + ".1", m16 + j * stride, B, td, &mrec[j]);
+        if (m == nullptr) {
+          m = mj;
+        } else {
+          add_f32(m, m, mj, n, E.st);
+          E.rel(mj);
+        }
+      }
       add_f32(t, t, m, n, E.st);
       E.rel(m);
     }
@@ -1569,7 +1627,8 @@ struct Net {
       float* dt = E.alloc<float>(n);
       silu_bwd(ls->temb, ls->dstemb, dt, n, 0, E.st);
       embed_mlp_bwd(Lp->pre + "temb_layer1", Lp->pre + "temb_layer2", trec, dt, B, td);
-      if (micro) embed_mlp_bwd(Lp->pre + "cond_layers.scale.0", Lp->pre + "cond_layers.scale.1", mrec, dt, B, td);
+      for (int j = 0; j < nkeys; ++j)
+        embed_mlp_bwd(Lp->micro_pre[j] + ".0", Lp->micro_pre[j] + ".1", mrec[j], dt, B, td);
       if (cs.cemb != nullptr) {
         if (cs.dcemb == nullptr) cs.dcemb = E.zeros_f32(static_cast<long long>(cs.B) * td);  // whole batch
         axpy_f32(cs.dcemb, dt, 1.f, n, 1, E.st);  // this level's leading rows
@@ -1949,7 +2008,8 @@ struct Net {
   // pool; pool addresses, TMA descriptors and gradient pointers are baked into the graph, so anything that moves them
   // (rebinding parameters, the pool returning memory to the driver) drops the recorded graphs.
   struct GraphRec {
-    int training = 0, batch = 0, tokens = 0, has_mask = 0, has_micro = 0, apply_lm_mask = 0, dropout = 0;
+    int training = 0, batch = 0, tokens = 0, has_mask = 0, apply_lm_mask = 0, dropout = 0;
+    int micro_mask = 0;  // bit k: the micro table's key k has values (staged in micro[k])
     int stage = 0, cond_cache = 0, has_cemb = 0;  // stage 2: the K/V cache mode and whether cond_emb is given
     uint64_t kv_epoch = 0;
     int lb[MDM_MAX_LEVELS] = {0, 0, 0, 0}, res[MDM_MAX_LEVELS] = {0, 0, 0, 0};
@@ -1959,7 +2019,8 @@ struct Net {
     float* dout[MDM_MAX_LEVELS] = {nullptr, nullptr, nullptr, nullptr};
     size_t x_bytes[MDM_MAX_LEVELS] = {0, 0, 0, 0};
     long long* times = nullptr;
-    float *lm = nullptr, *mask = nullptr, *micro = nullptr;  // mask: lm_mask (stage 0) or cross_mask (stage 2)
+    float *lm = nullptr, *mask = nullptr;  // mask: lm_mask (stage 0) or cross_mask (stage 2)
+    float* micro[MDM_MAX_MICRO] = {};
     size_t lm_bytes = 0, mask_bytes = 0;
     float *cond = nullptr, *cemb = nullptr, *dcond = nullptr, *dcemb = nullptr;  // stage 2
     size_t cond_bytes = 0, cemb_bytes = 0;
@@ -1998,17 +2059,23 @@ struct Net {
     cudaFree(r.times);
     cudaFree(r.lm);
     cudaFree(r.mask);
-    cudaFree(r.micro);
+    for (float* m : r.micro) cudaFree(m);
     cudaFree(r.cond);
     cudaFree(r.cemb);
     cudaFree(r.dcond);
     cudaFree(r.dcemb);
   }
   static const float* key_mask(const StepIO* q) { return q->stage == 2 ? q->cross_mask : q->lm_mask; }
+  int micro_mask(const StepIO* q) const {
+    int m = 0;
+    for (int k = 0; k < micro.num_keys; ++k)
+      if (q->values[k] != nullptr) m |= 1 << k;
+    return m;
+  }
   bool same_key(const GraphRec& r, const StepIO* q) const {
     if (r.training != (q->save_for_backward != 0) || r.batch != q->batch || r.tokens != q->tokens ||
         r.apply_lm_mask != (q->apply_lm_mask != 0) || r.dropout != (q->dropout != 0) ||
-        r.has_mask != (key_mask(q) != nullptr) || r.has_micro != (q->micro_scale != nullptr) || r.stage != q->stage ||
+        r.has_mask != (key_mask(q) != nullptr) || r.micro_mask != micro_mask(q) || r.stage != q->stage ||
         r.cond_cache != q->cond_cache || r.has_cemb != (q->stage == 2 && q->cond_emb != nullptr))
       return false;
     for (int l = 0; l < cfg.num_levels; ++l)
@@ -2030,7 +2097,7 @@ struct Net {
     r.batch = q->batch;
     r.tokens = q->tokens;
     r.has_mask = key_mask(q) != nullptr;
-    r.has_micro = q->micro_scale != nullptr;
+    r.micro_mask = micro_mask(q);
     r.stage = q->stage;
     r.cond_cache = q->cond_cache;
     r.has_cemb = q->stage == 2 && q->cond_emb != nullptr;
@@ -2063,7 +2130,8 @@ struct Net {
       r.mask_bytes = sizeof(float) * static_cast<size_t>(r.batch) * r.tokens;
       MDM_CUDA(cudaMalloc(&r.mask, r.mask_bytes));
     }
-    if (r.has_micro) MDM_CUDA(cudaMalloc(&r.micro, sizeof(float) * r.batch));
+    for (int k = 0; k < micro.num_keys; ++k)
+      if ((r.micro_mask >> k) & 1) MDM_CUDA(cudaMalloc(&r.micro[k], sizeof(float) * r.batch));
     graphs.push_back(r);
     return static_cast<int>(graphs.size()) - 1;
   }
@@ -2124,8 +2192,9 @@ struct Net {
     if (r.has_mask) MDM_CUDA(cudaMemcpyAsync(r.mask, key_mask(io_), r.mask_bytes, cudaMemcpyDeviceToDevice, st));
     if (r.cond != nullptr) MDM_CUDA(cudaMemcpyAsync(r.cond, io_->cond, r.cond_bytes, cudaMemcpyDeviceToDevice, st));
     if (r.cemb != nullptr) MDM_CUDA(cudaMemcpyAsync(r.cemb, io_->cond_emb, r.cemb_bytes, cudaMemcpyDeviceToDevice, st));
-    if (r.has_micro)
-      MDM_CUDA(cudaMemcpyAsync(r.micro, io_->micro_scale, sizeof(float) * r.batch, cudaMemcpyDeviceToDevice, st));
+    for (int k = 0; k < micro.num_keys; ++k)
+      if (r.micro[k] != nullptr)
+        MDM_CUDA(cudaMemcpyAsync(r.micro[k], io_->values[k], sizeof(float) * r.batch, cudaMemcpyDeviceToDevice, st));
     eng.st = st;
     prepare_weights();  // outside the graph: only runs when the fp32 masters changed
     const bool valid = r.fwd != nullptr && r.bind_epoch == bind_epoch && r.pool_epoch == eng.pool.epoch() &&
@@ -2148,7 +2217,7 @@ struct Net {
       } else {
         sio.lm_mask = r.has_mask ? r.mask : nullptr;
       }
-      sio.micro_scale = r.has_micro ? r.micro : nullptr;
+      for (int k = 0; k < MDM_MAX_MICRO; ++k) sio.values[k] = r.micro[k];
       const unsigned long long k0 = g_launch_count;
       MDM_CUDA(cudaStreamBeginCapture(cap_st, cudaStreamCaptureModeRelaxed));
       try {
@@ -2342,6 +2411,21 @@ struct mdm_net {
 extern "C" {
 
 int mdm_net_create(const mdm_net_cfg* cfg, mdm_net** out) {
+  // the one-key table {"scale": micro_scale_default} of every level that sets has_micro_scale
+  mdm_micro_cfg m{};
+  mdm_net_cfg c = *cfg;
+  for (int l = 0; l < std::min<int>(c.num_levels, MDM_MAX_LEVELS); ++l) {
+    if (!c.levels[l].has_micro_scale) continue;
+    m.num_keys = 1;
+    strcpy(m.names[0], "scale");
+    m.level_num_keys[l] = 1;
+    m.level_defaults[l][0] = c.levels[l].micro_scale_default;
+    c.levels[l].has_micro_scale = 0;
+  }
+  return mdm_net_create_micro(&c, &m, out);
+}
+
+int mdm_net_create_micro(const mdm_net_cfg* cfg, const mdm_micro_cfg* micro, mdm_net** out) {
   MDM_TRY({
     int dev = 0, major = 0, minor = 0;
     MDM_CUDA(cudaGetDevice(&dev));
@@ -2351,6 +2435,7 @@ int mdm_net_create(const mdm_net_cfg* cfg, mdm_net** out) {
       throw mdm::MdmFail("mdm_b200 requires an sm_90a (H100) device; there is no fallback path");
     auto* n = new mdm_net();
     n->net.cfg = *cfg;
+    if (micro != nullptr) n->net.micro = *micro;
     try {
       n->net.build();
     } catch (...) {
@@ -2432,14 +2517,34 @@ int mdm_net_forward(mdm_net* net, const mdm_net_io* io, mdm_stream_t stream) {
   return mdm_net_forward_stage(net, io, nullptr, stream);
 }
 
-int mdm_net_forward_stage(mdm_net* net, const mdm_net_io* io, const mdm_net_stage_io* stage, mdm_stream_t stream) {
+static int forward_with(mdm_net* net, const mdm_net_io* io, const mdm_net_stage_io* stage, const mdm_net_micro_io& micro,
+                        mdm_stream_t stream) {
   MDM_TRY({
     mdm::StepIO q{};
     static_cast<mdm_net_io&>(q) = *io;
+    q.micro_scale = nullptr;
     if (stage != nullptr) static_cast<mdm_net_stage_io&>(q) = *stage;
+    for (int k = 0; k < net->net.micro.num_keys; ++k) q.values[k] = micro.values[k];
     net->net.forward(&q, static_cast<cudaStream_t>(stream));
     MDM_CUDA(cudaGetLastError());
   })
+}
+
+int mdm_net_forward_stage(mdm_net* net, const mdm_net_io* io, const mdm_net_stage_io* stage, mdm_stream_t stream) {
+  mdm_net_micro_io m{};
+  if (net->net.scale_slot >= 0) m.values[net->net.scale_slot] = io->micro_scale;
+  return forward_with(net, io, stage, m, stream);
+}
+
+int mdm_net_forward_micro(mdm_net* net, const mdm_net_io* io, const mdm_net_stage_io* stage,
+                          const mdm_net_micro_io* micro, mdm_stream_t stream) {
+  if (io->micro_scale != nullptr) {
+    mdm::set_error("mdm_net_forward_micro: io->micro_scale must be NULL (pass the key \"scale\" in micro->values)");
+    return -1;
+  }
+  mdm_net_micro_io m{};
+  if (micro != nullptr) m = *micro;
+  return forward_with(net, io, stage, m, stream);
 }
 
 int mdm_net_backward(mdm_net* net, const mdm_net_grad_io* gio, mdm_stream_t stream) {

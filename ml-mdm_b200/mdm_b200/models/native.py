@@ -9,6 +9,7 @@ import torch
 from .. import _lib
 
 MAX_RES, MAX_LEVELS = 8, 4
+MAX_MICRO, MICRO_NAME_LEN = 8, 32  # MDM_MAX_MICRO, MDM_MICRO_NAME_LEN
 
 
 class LevelCfg(C.Structure):
@@ -78,6 +79,23 @@ class StageIO(C.Structure):
     ]
 
 
+class MicroCfg(C.Structure):
+    """mdm_micro_cfg: the nest's micro-conditioning keys (first appearance, outermost level first) and each level's
+    keys, as indices into that table in the level's order, with their defaults."""
+    _fields_ = [
+        ("num_keys", C.c_int32),
+        ("names", (C.c_char * MICRO_NAME_LEN) * MAX_MICRO),
+        ("level_num_keys", C.c_int32 * MAX_LEVELS),
+        ("level_keys", (C.c_int32 * MAX_MICRO) * MAX_LEVELS),
+        ("level_defaults", (C.c_float * MAX_MICRO) * MAX_LEVELS),
+    ]
+
+
+class MicroIO(C.Structure):
+    """mdm_net_micro_io: (batch,) fp32 values per table key, NULL = the levels' defaults."""
+    _fields_ = [("values", C.c_void_p * MAX_MICRO)]
+
+
 class NetGradIO(C.Structure):
     _fields_ = [
         ("dout", C.c_void_p * MAX_LEVELS),
@@ -106,6 +124,7 @@ def build_net_cfg(module) -> NetCfg:
     mods = module._levels()
     nc = NetCfg()
     nc.num_levels = len(cfgs)
+    scale_only = _scale_only(mods)
     for li, (cfg, m) in enumerate(zip(cfgs, mods)):
         lc = nc.levels[li]
         ch = _ints(cfg.resolution_channels)
@@ -126,8 +145,10 @@ def build_net_cfg(module) -> NetCfg:
         lc.skip_mid_blocks = int(bool(cfg.skip_mid_blocks))
         lc.nesting = int(bool(cfg.nesting))
         lc.skip_normalization = int(bool(getattr(cfg, "skip_normalization", True)))
-        lc.has_micro_scale = int(m.conditions is not None)
-        lc.micro_scale_default = float(m.conditions["scale"]) if m.conditions is not None else 0.0
+        # "scale:<default>" nests keep the one-key fields of mdm_net_create; any other keys go in build_micro_cfg's table
+        if scale_only:
+            lc.has_micro_scale = int(m.conditions is not None)
+            lc.micro_scale_default = float(m.conditions["scale"]) if m.conditions is not None else 0.0
         lc.dropout = float(cfg.resnet_config.dropout)
     inner = mods[-1]
     icfg = cfgs[-1]
@@ -141,6 +162,32 @@ def build_net_cfg(module) -> NetCfg:
     nc.num_heads = 8
     nc.num_lm_head_layers = len(inner.lm_head) if getattr(inner, "lm_head", None) is not None else 0
     return nc
+
+
+def _scale_only(mods):
+    return all(m.conditions is None or list(m.conditions) == ["scale"] for m in mods)
+
+
+def build_micro_cfg(module) -> MicroCfg:
+    """The micro-conditioning table of the nest (mdm_net_create_micro) from every level's `conditions`."""
+    mc = MicroCfg()
+    names = []
+    for li, m in enumerate(module._levels()):
+        conds = m.conditions or {}
+        for j, (key, default) in enumerate(conds.items()):
+            if key not in names:
+                if len(names) == MAX_MICRO:
+                    raise _lib.MdmError(f"micro_conditioning: the nest has more than {MAX_MICRO} distinct keys")
+                raw = key.encode()
+                if len(raw) >= MICRO_NAME_LEN:
+                    raise _lib.MdmError(f"micro_conditioning key '{key}' is longer than {MICRO_NAME_LEN - 1} bytes")
+                mc.names[len(names)].value = raw
+                names.append(key)
+            mc.level_keys[li][j] = names.index(key)
+            mc.level_defaults[li][j] = float(default)
+        mc.level_num_keys[li] = len(conds)
+    mc.num_keys = len(names)
+    return mc
 
 
 class _DenoiseFn(torch.autograd.Function):
@@ -227,7 +274,13 @@ class NativeNet:
         self.lib = _lib.lib()
         self.cfg = build_net_cfg(module)
         self.handle = C.c_void_p()
-        _lib.check(self.lib.mdm_net_create(C.byref(self.cfg), C.byref(self.handle)), "mdm_net_create")
+        self.micro_cfg = build_micro_cfg(module)
+        self.micro_keys = [self.micro_cfg.names[k].value.decode() for k in range(self.micro_cfg.num_keys)]
+        if _scale_only(module._levels()):
+            _lib.check(self.lib.mdm_net_create(C.byref(self.cfg), C.byref(self.handle)), "mdm_net_create")
+        else:
+            _lib.check(self.lib.mdm_net_create_micro(C.byref(self.cfg), C.byref(self.micro_cfg), C.byref(self.handle)),
+                       "mdm_net_create_micro")
         self.lib.mdm_net_workspace_bytes.restype = C.c_uint64
         self.lib.mdm_net_workspace_high_water.restype = C.c_uint64
         self.lib.mdm_net_debug_fetch.restype = C.c_int64
@@ -355,7 +408,7 @@ class NativeNet:
     def run(self, xs, times, lm, mask, micros, apply_lm_mask=False):
         self._bind()
         self.apply_lm_mask = bool(apply_lm_mask)
-        micro = self._enter(micros)
+        micro = self._enter(micros, xs[-1].shape[0])
         # (Function.forward runs with grad mode off, so the decision is taken here)
         need_grad = torch.is_grad_enabled() and any(p.requires_grad for p in self.params)
         return _DenoiseFn.apply(self, len(xs), need_grad, times, lm, mask, micro, *xs, *self.params)
@@ -376,7 +429,7 @@ class NativeNet:
         """forward_denoising on the engine (stage 2). Without autograd the K/V the cross-attention blocks compute from
         `cond` are kept by the engine and reused while `cond`, `cross_mask` and the weights stay what they were."""
         self._bind()
-        micro = self._enter(micros)
+        micro = self._enter(micros, xs[-1].shape[0])
         need_grad = torch.is_grad_enabled() and (any(p.requires_grad for p in self.params) or any(
             t is not None and t.requires_grad for t in (cond, cond_emb)))
         if self.cfg.cond_dim > 0 and cond is None:
@@ -411,11 +464,23 @@ class NativeNet:
         ok = same(old[0], new[0]) and same(old[1], new[1]) and old[2:] == new[2:]
         return 2 if ok else 1
 
-    def _enter(self, micros):
-        """micro-conditioning tensor and the dropout (flag, seed) of the forward being entered."""
-        micro = None
-        if micros:
-            micro = micros.get("scale", None)
+    def _enter(self, micros, batch):
+        """The micro-conditioning values of the forward being entered, one (batch,) fp32 tensor or None per key of the
+        engine's table (keys no level configures are ignored, as the reference ignores them), and its dropout
+        (flag, seed). A one-element value is broadcast over the batch, as torch broadcasting does in the reference."""
+        micro = []
+        for key in self.micro_keys:
+            v = micros.get(key) if micros else None
+            if v is not None:
+                if not isinstance(v, torch.Tensor):
+                    raise _lib.MdmError(f"micro-conditioning value '{key}' must be a CUDA tensor")
+                if v.numel() not in (1, batch):
+                    raise _lib.MdmError(f"micro-conditioning value '{key}' has {v.numel()} elements; the batch is "
+                                        f"{batch} (one value per sample, or one for all)")
+                if not v.is_cuda:
+                    raise _lib.MdmError(f"micro-conditioning value '{key}' must be a CUDA tensor")
+                v = v.detach().reshape(-1).float().expand(batch).contiguous()
+            micro.append(v)
         self.dropout = (0, 0)
         if self.max_dropout > 0:
             training = self.module.training
@@ -484,9 +549,11 @@ class NativeNet:
                 sio.cond_emb = f32(cond_emb).data_ptr()
             if cross_mask is not None:
                 sio.cross_mask = f32(cross_mask).data_ptr()
-        if micro is not None:
-            micro = f32(micro)
-            io.micro_scale = micro.data_ptr()
+        mio = MicroIO()
+        for k, v in enumerate(micro):
+            if v is not None:
+                keep.append(v)
+                mio.values[k] = v.data_ptr()
         io.save_for_backward = int(save)
         if stage == 2 and save:
             td = self.cfg.levels[self.cfg.num_levels - 1].temporal_dim
@@ -494,11 +561,8 @@ class NativeNet:
         io.apply_lm_mask = int(bool(apply_lm_mask))
         io.dropout, io.dropout_seed = self.dropout
         st = torch.cuda.current_stream().cuda_stream
-        if stage == 0:
-            _lib.check(self.lib.mdm_net_forward(self.handle, C.byref(io), C.c_void_p(st)), "mdm_net_forward")
-        else:
-            _lib.check(self.lib.mdm_net_forward_stage(self.handle, C.byref(io), C.byref(sio), C.c_void_p(st)),
-                       "mdm_net_forward_stage")
+        _lib.check(self.lib.mdm_net_forward_micro(self.handle, C.byref(io), C.byref(sio) if stage else None,
+                                                  C.byref(mio), C.c_void_p(st)), "mdm_net_forward_micro")
         self._keep = keep if save else None  # inputs must outlive the tape
         return outs
 

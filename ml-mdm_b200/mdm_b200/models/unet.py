@@ -18,7 +18,7 @@ import torch
 import torch.nn as nn
 
 from .. import _lib
-from .native import NativeNet
+from .native import MAX_MICRO, MICRO_NAME_LEN, NativeNet
 
 
 def zero_module(module):
@@ -40,6 +40,18 @@ def _ints(v, n=None):
     if n is not None and len(v) == 1:
         v = v * n
     return v
+
+
+def check_micro_conditions(conditions):
+    """What the engine accepts of one level's micro-conditioning keys ({key: default}, unet.py:615-620)."""
+    if len(conditions) > MAX_MICRO:
+        raise ValueError(f"micro_conditioning: {len(conditions)} keys, the native path takes at most {MAX_MICRO}")
+    for key, default in conditions.items():
+        if len(key.encode()) >= MICRO_NAME_LEN:
+            raise ValueError(f"micro_conditioning key '{key}' is longer than {MICRO_NAME_LEN - 1} bytes")
+        if key == "scale" and default == 0:
+            # the reference computes (micro / default).clamp(max=1) * default (unet.py:926): 0/0
+            raise ValueError("micro_conditioning key 'scale' needs a non-zero default")
 
 
 class _ResNet(nn.Module):
@@ -165,8 +177,7 @@ class UNet(nn.Module):
         if config.micro_conditioning is not None:
             self.conditions = {c.split(":")[0]: float(c.split(":")[1])
                                for c in config.micro_conditioning.split(",")}
-            if list(self.conditions) != ["scale"]:
-                raise NotImplementedError("only the 'scale' micro-conditioning of the shipped configs is built")
+            check_micro_conditions(self.conditions)
             self.cond_layers = nn.ModuleDict({
                 k: nn.ModuleList([nn.Linear(td // 4, td), zero_module(nn.Linear(td, td))])
                 for k in self.conditions})
