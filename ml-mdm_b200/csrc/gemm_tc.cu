@@ -4,6 +4,9 @@
 #include <stdio.h>
 #include <stdlib.h>
 
+#include <algorithm>
+#include <climits>
+#include <set>
 #include <utility>
 #include <vector>
 
@@ -35,6 +38,7 @@ constexpr int SMEM_LIMIT = 226 * 1024;  // dynamic shared memory; with the stati
 
 // warpgroup 0: TMA producer (one thread); warpgroups 1 and 2: wgmma consumers, 64 tile rows each, and the epilogue
 constexpr int NUM_THREADS = 384;
+constexpr int RASTER_N = 8;   // column tiles per band of the persistent kernel's tile order
 
 // Epilogue of one pair of adjacent columns (c, c + 1) of tile row r: alpha, bias, residual, GELU', then the stores.
 __device__ __forceinline__ void epi_pair(const GemmParams& p, long long row_off, int col0, float v0, float v1,
@@ -90,11 +94,160 @@ __device__ __forceinline__ void epi_pair(const GemmParams& p, long long row_off,
   }
 }
 
-template <bool A_MN, bool B_MN, int BN>
+// Operand planes a kernel multiplies besides A x B: the lo plane of B (weights) and the lo plane of a K-major A.
+constexpr int PL_BLO = 1;
+constexpr int PL_ALO = 2;
+
+// Stage layout of the plain and conv modes: A | B | B lo plane (PL_BLO) | A lo plane (PL_ALO).
+template <bool B_MN, int BN, int PL>
+struct StageLayout {
+  static constexpr int nb_alloc = B_MN ? ((BN + 63) / 64) * 64 : BN;
+  static constexpr int b_bytes = nb_alloc * 128;  // one B plane
+  static constexpr int b_lo_off = A_STAGE_BYTES + b_bytes;
+  static constexpr int a_lo_off = A_STAGE_BYTES + b_bytes * ((PL & PL_BLO) ? 2 : 1);
+  static constexpr int bytes = a_lo_off + ((PL & PL_ALO) ? A_STAGE_BYTES : 0);
+};
+
+// TMA loads of k block kb of the plain and conv modes into the stage at sA (producer thread).
+template <bool A_MN, bool B_MN, int BN, int PL>
+__device__ __forceinline__ void load_stage(const GemmParams& p, const CUtensorMap* tmA, const CUtensorMap* tmB,
+                                           const CUtensorMap* tmBlo, const CUtensorMap* tmAlo, uint8_t* sA,
+                                           uint64_t* bar, int kb, int m0, int n0, int z1, int z2, int img, int th,
+                                           int tw) {
+  using S = StageLayout<B_MN, BN, PL>;
+  constexpr int nslab_b = S::nb_alloc / 64;
+  uint8_t* sB = sA + A_STAGE_BYTES;
+  if (p.kind == GEMM_PLAIN) {
+    const int az1 = p.a_use_z ? z1 + p.a_z1_off : 0;
+    const int az2 = p.a_use_z ? z2 : 0;
+    const int bz1 = p.b_use_z ? z1 + p.b_z1_off : 0;
+    const int bz2 = p.b_use_z ? z2 : 0;
+    if (!A_MN) {
+      tma_load_4d(sA, tmA, bar, kb * BLOCK_K, m0, az1, az2);
+      if (PL & PL_ALO) tma_load_4d(sA + S::a_lo_off, tmAlo, bar, kb * BLOCK_K, m0, az1, az2);
+    } else {
+      tma_load_4d(sA, tmA, bar, m0, kb * BLOCK_K, az1, az2);
+      tma_load_4d(sA + SLAB_BYTES, tmA, bar, m0 + 64, kb * BLOCK_K, az1, az2);
+    }
+#pragma unroll
+    for (int pl = 0; pl <= ((PL & PL_BLO) ? 1 : 0); ++pl) {
+      const CUtensorMap* mb = pl ? tmBlo : tmB;
+      uint8_t* sBp = sB + pl * S::b_bytes;
+      if (!B_MN) {
+        tma_load_4d(sBp, mb, bar, kb * BLOCK_K, n0, bz1, bz2);
+      } else {
+        for (int s = 0; s < nslab_b; ++s)
+          tma_load_4d(sBp + s * SLAB_BYTES, mb, bar, n0 + 64 * s, kb * BLOCK_K, bz1, bz2);
+      }
+    }
+  } else {  // GEMM_CONV
+    const int tap = kb / p.kblocks_c;
+    const int cb = kb - tap * p.kblocks_c;
+    const int kh = (p.taps == 9) ? tap / 3 : 1;
+    const int kw = (p.taps == 9) ? tap % 3 : 1;
+    tma_load_4d(sA, tmA, bar, cb * BLOCK_K, tw * p.PW + kw - 1, th * p.PH + kh - 1, img);
+    if (PL & PL_ALO) tma_load_4d(sA + S::a_lo_off, tmAlo, bar, cb * BLOCK_K, tw * p.PW + kw - 1, th * p.PH + kh - 1, img);
+    const int wt = p.flip ? (p.taps - 1 - tap) : tap;
+#pragma unroll
+    for (int pl = 0; pl <= ((PL & PL_BLO) ? 1 : 0); ++pl) {
+      const CUtensorMap* mb = pl ? tmBlo : tmB;
+      uint8_t* sBp = sB + pl * S::b_bytes;
+      if (!B_MN) {
+        tma_load_4d(sBp, mb, bar, cb * BLOCK_K, n0, tap, 0);
+      } else {
+        for (int s = 0; s < nslab_b; ++s)
+          tma_load_4d(sBp + s * SLAB_BYTES, mb, bar, n0 + 64 * s, cb * BLOCK_K, wt, 0);
+      }
+    }
+  }
+}
+
+// The wgmmas of k16 step k of a plain / conv stage for 64 tile rows, in the order every output element sums them:
+// A x B, then A x B lo, then A lo x B. a_rows / a_lo_rows: those rows of the A planes in the stage.
+template <bool A_MN, bool B_MN, int BN, int PL>
+__device__ __forceinline__ void mma_k16(float* acc, uint32_t a_rows, uint32_t a_lo_rows, uint32_t b_base,
+                                        uint32_t b_lo_base, int k, uint32_t scale_d) {
+  const uint64_t adesc = A_MN ? make_smem_desc_sw128(a_rows + k * 2048, SLAB_BYTES, 1024)
+                              : make_smem_desc_sw128(a_rows + k * 32, 16, 1024);
+  const uint64_t bdesc = B_MN ? make_smem_desc_sw128(b_base + k * 2048, SLAB_BYTES, 1024)
+                              : make_smem_desc_sw128(b_base + k * 32, 16, 1024);
+  Wgmma<BN>::template ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc, scale_d);
+  if constexpr ((PL & PL_BLO) != 0) {
+    const uint64_t bdesc_lo = B_MN ? make_smem_desc_sw128(b_lo_base + k * 2048, SLAB_BYTES, 1024)
+                                   : make_smem_desc_sw128(b_lo_base + k * 32, 16, 1024);
+    Wgmma<BN>::template ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc_lo, 1u);
+  }
+  if constexpr (!A_MN && (PL & PL_ALO) != 0) {
+    Wgmma<BN>::template ss<0, B_MN ? 1 : 0>(acc, make_smem_desc_sw128(a_lo_rows + k * 32, 16, 1024), bdesc, 1u);
+  }
+}
+
+// Output tile of a linear tile index of the plain and conv modes (tiles ordered m fastest, then n, then z).
+struct TileCoord {
+  int m0, n0, z1, z2, img, th, tw, kb_begin, kb_end;
+};
+__device__ __forceinline__ TileCoord tile_coord(const GemmParams& p, int m_tile, int n_tile, int z, int bn) {
+  TileCoord c;
+  const int split = z % p.nsplit;
+  z /= p.nsplit;
+  c.z1 = z % p.nz1;
+  c.z2 = z / p.nz1;
+  const int per = (p.num_kblocks + p.nsplit - 1) / p.nsplit;
+  c.kb_begin = split * per;
+  c.kb_end = min(p.num_kblocks, c.kb_begin + per);
+  c.m0 = m_tile * BLOCK_M;
+  c.n0 = n_tile * bn;
+  c.img = c.th = c.tw = 0;
+  if (p.kind == GEMM_CONV) {
+    c.tw = m_tile % p.tiles_w;
+    const int t = m_tile / p.tiles_w;
+    c.th = t % p.tiles_h;
+    c.img = t / p.tiles_h;
+  }
+  return c;
+}
+
+// Epilogue of 64 tile rows (r0 .. r0 + 63) from the accumulators of one m64 wgmma.
+template <int BN>
+__device__ __forceinline__ void store_rows(const GemmParams& p, const float* acc, const TileCoord& c, int r0,
+                                           float alpha) {
+  const int lane = threadIdx.x & 31;
+  const int wq = (threadIdx.x >> 5) & 3;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = r0 + wq * 16 + (lane >> 2) + 8 * h;  // tile row of accumulator elements 4j + 2h + {0, 1}
+    bool valid;
+    long long row_off;
+    if (p.kind == GEMM_CONV) {
+      const int ph = r / p.PW;
+      const int pw = r - ph * p.PW;
+      const int hh = c.th * p.PH + ph;
+      const int ww = c.tw * p.PW + pw;
+      valid = (hh < p.H) && (ww < p.W) && (c.img < p.nimg);
+      row_off = (static_cast<long long>(c.img * p.H + hh) * p.W + ww) * p.ldc;
+    } else {
+      const int row = c.m0 + r;
+      valid = row < p.M;
+      row_off = static_cast<long long>(row) * p.ldc + static_cast<long long>(c.z1) * p.c_z1_stride +
+                static_cast<long long>(c.z2) * p.c_z2_stride;
+    }
+    if (!valid) continue;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+      epi_pair(p, row_off, c.n0 + j * 8 + (lane & 3) * 2, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], alpha);
+  }
+}
+
+__device__ __forceinline__ float epi_alpha(const GemmParams& p) {
+  return p.alpha_dev != nullptr ? p.alpha * __ldg(p.alpha_dev) : p.alpha;
+}
+
+// One output tile per CTA: the weight gradients (MN-major A: plain MN x MN with split-K, 3x3 wgrad with tall stages).
+template <bool B_MN, int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmBlo, const int b_split, const __grid_constant__ CUtensorMap tmAlo,
-               const int a_split, const GemmParams p) {
+               const __grid_constant__ CUtensorMap tmBlo, const __grid_constant__ CUtensorMap tmAlo,
+               const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[MAX_STAGES];
   __shared__ __align__(8) uint64_t empty_bar[MAX_STAGES];
@@ -103,45 +256,21 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                                              ~static_cast<uintptr_t>(1023));
   const int wg = threadIdx.x >> 7;
 
-  constexpr int nb_alloc = B_MN ? ((BN + 63) / 64) * 64 : BN;
+  using S = StageLayout<B_MN, BN, 0>;
   // weight gradients of narrow layers: kf x 64 pixel rows per stage, and a single A slab when M <= 64
   const int kf = (p.kind == GEMM_CONV_WGRAD && p.kfactor > 1) ? p.kfactor : 1;
   const int slab_bytes = SLAB_BYTES * kf;
   const int a_slabs = (kf > 1 && p.M <= 64) ? 1 : 2;
   const int a_stage_bytes = kf > 1 ? a_slabs * slab_bytes : A_STAGE_BYTES;
-  const int b_stage_bytes = nb_alloc * 128 * kf;  // one B plane; a split B stages its lo plane right behind it
-  // stage: A | B | B lo plane (split B) | A lo plane (split A, K-major)
-  const int a_lo_off = a_stage_bytes + b_stage_bytes * (b_split ? 2 : 1);
-  const int stage_bytes = a_lo_off + (a_split ? a_stage_bytes : 0);
+  const int stage_bytes = kf > 1 ? a_stage_bytes + S::nb_alloc * 128 * kf : S::bytes;
   const int nstages = p.num_stages;
 
-  // ---- block coordinates
-  int z = blockIdx.z;
-  const int split = z % p.nsplit;
-  z /= p.nsplit;
-  const int z1 = z % p.nz1;
-  const int z2 = z / p.nz1;
-  const int per = (p.num_kblocks + p.nsplit - 1) / p.nsplit;
-  const int kb_begin = split * per;
-  const int kb_end = min(p.num_kblocks, kb_begin + per);
-  const int nkb = kb_end - kb_begin;
-
-  const int m_tile = blockIdx.x;
-  const int m0 = m_tile * BLOCK_M;
-  const int n0 = blockIdx.y * BN;
-  int img = 0, th = 0, tw = 0;
-  if (p.kind == GEMM_CONV) {
-    tw = m_tile % p.tiles_w;
-    const int t = m_tile / p.tiles_w;
-    th = t % p.tiles_h;
-    img = t / p.tiles_h;
-  }
+  const TileCoord c = tile_coord(p, blockIdx.x, blockIdx.y, blockIdx.z, BN);
+  const int nkb = c.kb_end - c.kb_begin;
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
-    if (b_split) prefetch_tmap(&tmBlo);
-    if (a_split) prefetch_tmap(&tmAlo);
     for (int s = 0; s < nstages; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 8);  // one arrival per consumer warp
@@ -156,65 +285,28 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      const int az1 = p.a_use_z ? z1 + p.a_z1_off : 0;
-      const int az2 = p.a_use_z ? z2 : 0;
-      const int bz1 = p.b_use_z ? z1 + p.b_z1_off : 0;
-      const int bz2 = p.b_use_z ? z2 : 0;
-      constexpr int nslab_b = nb_alloc / 64;
       for (int i = 0; i < nkb; ++i) {
-        const int kb = kb_begin + i;
+        const int kb = c.kb_begin + i;
         mbar_wait(&empty_bar[stage], phase ^ 1);
         uint8_t* sA = smem + stage * stage_bytes;
-        uint8_t* sB = sA + a_stage_bytes;
         uint64_t* bar = &full_bar[stage];
         mbar_expect_tx(bar, static_cast<uint32_t>(stage_bytes));
-        if (p.kind == GEMM_PLAIN) {
-          if (!A_MN) {
-            tma_load_4d(sA, &tmA, bar, kb * BLOCK_K, m0, az1, az2);
-            if (a_split) tma_load_4d(sA + a_lo_off, &tmAlo, bar, kb * BLOCK_K, m0, az1, az2);
-          } else {
-            tma_load_4d(sA, &tmA, bar, m0, kb * BLOCK_K, az1, az2);
-            tma_load_4d(sA + SLAB_BYTES, &tmA, bar, m0 + 64, kb * BLOCK_K, az1, az2);
-          }
-          for (int pl = 0; pl <= b_split; ++pl) {
-            const CUtensorMap* mb = pl ? &tmBlo : &tmB;
-            uint8_t* sBp = sB + pl * b_stage_bytes;
-            if (!B_MN) {
-              tma_load_4d(sBp, mb, bar, kb * BLOCK_K, n0, bz1, bz2);
-            } else {
-              for (int s = 0; s < nslab_b; ++s)
-                tma_load_4d(sBp + s * SLAB_BYTES, mb, bar, n0 + 64 * s, kb * BLOCK_K, bz1, bz2);
-            }
-          }
-        } else if (p.kind == GEMM_CONV) {
-          const int tap = kb / p.kblocks_c;
-          const int cb = kb - tap * p.kblocks_c;
-          const int kh = (p.taps == 9) ? tap / 3 : 1;
-          const int kw = (p.taps == 9) ? tap % 3 : 1;
-          tma_load_4d(sA, &tmA, bar, cb * BLOCK_K, tw * p.PW + kw - 1, th * p.PH + kh - 1, img);
-          if (a_split) tma_load_4d(sA + a_lo_off, &tmAlo, bar, cb * BLOCK_K, tw * p.PW + kw - 1, th * p.PH + kh - 1, img);
-          const int wt = p.flip ? (p.taps - 1 - tap) : tap;
-          for (int pl = 0; pl <= b_split; ++pl) {
-            const CUtensorMap* mb = pl ? &tmBlo : &tmB;
-            uint8_t* sBp = sB + pl * b_stage_bytes;
-            if (!B_MN) {
-              tma_load_4d(sBp, mb, bar, cb * BLOCK_K, n0, tap, 0);
-            } else {
-              for (int s = 0; s < nslab_b; ++s)
-                tma_load_4d(sBp + s * SLAB_BYTES, mb, bar, n0 + 64 * s, cb * BLOCK_K, wt, 0);
-            }
-          }
-        } else {  // GEMM_CONV_WGRAD: k block = one patch of 64 * kf pixels
+        if (p.kind != GEMM_CONV_WGRAD) {
+          load_stage<true, B_MN, BN, 0>(p, &tmA, &tmB, &tmBlo, &tmAlo, sA, bar, kb, c.m0, c.n0, c.z1, c.z2, c.img,
+                                         c.th, c.tw);
+        } else {  // k block = one patch of 64 * kf pixels
+          uint8_t* sB = sA + a_stage_bytes;
           const int ptw = kb % p.tiles_w;
           const int t = kb / p.tiles_w;
           const int pth = t % p.tiles_h;
           const int pimg = t / p.tiles_h;
-          const int kh = (p.taps == 9) ? z1 / 3 : 1;
-          const int kw = (p.taps == 9) ? z1 % 3 : 1;
-          tma_load_4d(sA, &tmA, bar, m0, ptw * p.PW, pth * p.PH, pimg);
-          if (a_slabs == 2) tma_load_4d(sA + slab_bytes, &tmA, bar, m0 + 64, ptw * p.PW, pth * p.PH, pimg);
-          for (int s = 0; s < nslab_b; ++s)
-            tma_load_4d(sB + s * slab_bytes, &tmB, bar, n0 + 64 * s, ptw * p.PW + kw - 1, pth * p.PH + kh - 1, pimg);
+          const int kh = (p.taps == 9) ? c.z1 / 3 : 1;
+          const int kw = (p.taps == 9) ? c.z1 % 3 : 1;
+          tma_load_4d(sA, &tmA, bar, c.m0, ptw * p.PW, pth * p.PH, pimg);
+          if (a_slabs == 2) tma_load_4d(sA + slab_bytes, &tmA, bar, c.m0 + 64, ptw * p.PW, pth * p.PH, pimg);
+          for (int s = 0; s < S::nb_alloc / 64; ++s)
+            tma_load_4d(sB + s * slab_bytes, &tmB, bar, c.n0 + 64 * s, ptw * p.PW + kw - 1, pth * p.PH + kh - 1,
+                        pimg);
         }
         if (++stage == nstages) {
           stage = 0;
@@ -229,7 +321,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   reg_alloc<232>();
   const int cw = wg - 1;  // this warpgroup's 64 rows of the tile
   const int lane = threadIdx.x & 31;
-  const int wq = (threadIdx.x >> 5) & 3;
   float acc[BN / 2];
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
@@ -241,38 +332,25 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const uint32_t a_base = smem_u32(smem + stage * stage_bytes);
       const uint32_t b_base = a_base + a_stage_bytes;
       fence_regs<BN / 2>(acc);
-      wgmma_arrive();
-      if (kf == 1) {
-        const uint32_t a_wg = A_MN ? a_base + cw * SLAB_BYTES : a_base + cw * 64 * 128;
-#pragma unroll
-        for (int k = 0; k < BLOCK_K / 16; ++k) {
-          const uint64_t adesc = A_MN ? make_smem_desc_sw128(a_wg + k * 2048, SLAB_BYTES, 1024)
-                                      : make_smem_desc_sw128(a_wg + k * 32, 16, 1024);
-          const uint64_t bdesc = B_MN ? make_smem_desc_sw128(b_base + k * 2048, SLAB_BYTES, 1024)
-                                      : make_smem_desc_sw128(b_base + k * 32, 16, 1024);
-          Wgmma<BN>::template ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc, (i > 0 || k > 0) ? 1u : 0u);
-          if (b_split) {
-            const uint32_t b_lo = b_base + b_stage_bytes;
-            const uint64_t bdesc_lo = B_MN ? make_smem_desc_sw128(b_lo + k * 2048, SLAB_BYTES, 1024)
-                                           : make_smem_desc_sw128(b_lo + k * 32, 16, 1024);
-            Wgmma<BN>::template ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc_lo, 1u);
-          }
-          if (!A_MN && a_split) {
-            const uint64_t adesc_lo = make_smem_desc_sw128(a_base + a_lo_off + cw * 64 * 128 + k * 32, 16, 1024);
-            Wgmma<BN>::template ss<0, B_MN ? 1 : 0>(acc, adesc_lo, bdesc, 1u);
-          }
-        }
-      } else if constexpr (A_MN && B_MN) {
-        // tall MN-major slabs (kf * 64 pixel rows x 64 columns). With one A slab (M <= 64) the second warpgroup
-        // re-reads the first slab: its rows (64..127) are never stored.
+      if constexpr (B_MN) {
+        // kf * 64 pixel rows x 64 columns per MN-major slab (64 rows outside the 3x3 wgrad). With one A slab
+        // (M <= 64) the second warpgroup re-reads the first slab: its rows (64..127) are never stored.
         const uint32_t a_wg = a_base + (a_slabs == 2 ? cw * slab_bytes : 0);
+        wgmma_arrive();
         for (int k = 0; k < 4 * kf; ++k) {
           const uint64_t adesc = make_smem_desc_sw128(a_wg + k * 2048, static_cast<uint32_t>(slab_bytes), 1024);
           const uint64_t bdesc = make_smem_desc_sw128(b_base + k * 2048, static_cast<uint32_t>(slab_bytes), 1024);
           Wgmma<BN>::template ss<1, 1>(acc, adesc, bdesc, (i > 0 || k > 0) ? 1u : 0u);
         }
+        wgmma_commit();
+      } else {
+        const uint32_t a_wg = a_base + cw * SLAB_BYTES;
+        wgmma_arrive();
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / 16; ++k)
+          mma_k16<true, false, BN, 0>(acc, a_wg, 0, b_base, 0, k, (i > 0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
       }
-      wgmma_commit();
       // the previous stage's MMAs have retired once at most this stage's group is in flight: free that slot
       wgmma_wait<1>();
       fence_regs<BN / 2>(acc);
@@ -288,30 +366,120 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
 
   // =========================== epilogue ===========================
-  float alpha = p.alpha;
-  if (p.alpha_dev != nullptr) alpha *= __ldg(p.alpha_dev);
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int r = cw * 64 + wq * 16 + (lane >> 2) + 8 * h;  // tile row of accumulator elements 4j + 2h + {0, 1}
-    bool valid;
-    long long row_off;
-    if (p.kind == GEMM_CONV) {
-      const int ph = r / p.PW;
-      const int pw = r - ph * p.PW;
-      const int hh = th * p.PH + ph;
-      const int ww = tw * p.PW + pw;
-      valid = (hh < p.H) && (ww < p.W) && (img < p.nimg);
-      row_off = (static_cast<long long>(img * p.H + hh) * p.W + ww) * p.ldc;
-    } else {
-      const int row = m0 + r;
-      valid = row < p.M;
-      row_off = static_cast<long long>(row) * p.ldc + static_cast<long long>(z1) * p.c_z1_stride +
-                static_cast<long long>(z2) * p.c_z2_stride;
+  store_rows<BN>(p, acc, c, cw * 64, epi_alpha(p));
+}
+
+// Persistent schedule of the weight products (plain K x K, plain K x MN, 3x3 conv forward / data gradient; K-major A,
+// BN <= 128). Each CTA walks tiles blockIdx.x + i * gridDim.x in the order of the one-tile grid, and the producer
+// streams the k blocks of all its tiles through one stage ring, so the next tile's stages load while the consumers
+// run the epilogue of the last one. Both consumer warpgroups work on every tile, 64 rows each, as in the one-tile
+// kernel. (Consumers taking alternate whole tiles, one in its epilogue while the other issues MMAs, measured slower:
+// at 128 accumulators per thread the epilogue of a whole tile on one warpgroup took more than twice as long.)
+template <bool B_MN, int BN, int PL>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                       const __grid_constant__ CUtensorMap tmBlo, const __grid_constant__ CUtensorMap tmAlo,
+                       const GemmParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ __align__(8) uint64_t full_bar[MAX_STAGES];
+  __shared__ __align__(8) uint64_t empty_bar[MAX_STAGES];
+
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  const int wg = threadIdx.x >> 7;
+  using S = StageLayout<B_MN, BN, PL>;
+  const int nstages = p.num_stages;
+  const int m_tiles = p.kind == GEMM_CONV ? p.nimg * p.tiles_h * p.tiles_w : (p.M + BLOCK_M - 1) / BLOCK_M;
+  const int n_tiles = (p.N + BN - 1) / BN;
+  const int num_tiles = m_tiles * n_tiles * p.nz1 * p.nz2 * p.nsplit;
+  // Tile order: bands of RASTER_N column tiles; within a band the band's columns fastest, then m. The CTAs resident at
+  // one time then cover ~132 / RASTER_N row tiles x RASTER_N column tiles, so A is read from HBM once per band instead
+  // of once per column tile. Each output element's sum is the same in any tile order.
+  auto coord = [&](int t) {
+    const int per_z = m_tiles * n_tiles;
+    const int z = t / per_z;
+    const int r = t - z * per_z;
+    const int band = r / (m_tiles * RASTER_N);
+    const int in_band = r - band * (m_tiles * RASTER_N);
+    const int width = min(RASTER_N, n_tiles - band * RASTER_N);
+    return tile_coord(p, in_band / width, band * RASTER_N + in_band % width, z, BN);
+  };
+
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&tmA);
+    prefetch_tmap(&tmB);
+    if (PL & PL_BLO) prefetch_tmap(&tmBlo);
+    if (PL & PL_ALO) prefetch_tmap(&tmAlo);
+    for (int s = 0; s < nstages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 8);  // one arrival per consumer warp
     }
-    if (!valid) continue;
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    // =========================== TMA producer ===========================
+    reg_dealloc<40>();
+    if (threadIdx.x == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+        const TileCoord c = coord(t);
+        for (int kb = c.kb_begin; kb < c.kb_end; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sA = smem + stage * S::bytes;
+          uint64_t* bar = &full_bar[stage];
+          mbar_expect_tx(bar, static_cast<uint32_t>(S::bytes));
+          load_stage<false, B_MN, BN, PL>(p, &tmA, &tmB, &tmBlo, &tmAlo, sA, bar, kb, c.m0, c.n0, c.z1, c.z2, c.img,
+                                          c.th, c.tw);
+          if (++stage == nstages) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // =========================== wgmma consumers ===========================
+  reg_alloc<232>();
+  const int cw = wg - 1;  // this warpgroup's 64 rows of every tile
+  const int lane = threadIdx.x & 31;
+  const float alpha = epi_alpha(p);
+  float acc[BN / 2];
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+    const TileCoord c = coord(t);
+    int prev = -1;
+    for (int i = c.kb_begin; i < c.kb_end; ++i) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t a_base = smem_u32(smem + stage * S::bytes);
+      fence_regs<BN / 2>(acc);
+      wgmma_arrive();
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j)
-      epi_pair(p, row_off, n0 + j * 8 + (lane & 3) * 2, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], alpha);
+      for (int k = 0; k < BLOCK_K / 16; ++k)
+        mma_k16<false, B_MN, BN, PL>(acc, a_base + cw * 64 * 128, a_base + S::a_lo_off + cw * 64 * 128,
+                                     a_base + A_STAGE_BYTES, a_base + S::b_lo_off, k,
+                                     (i > c.kb_begin || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      // the previous stage's MMAs have retired once at most this stage's group is in flight: free that slot
+      wgmma_wait<1>();
+      fence_regs<BN / 2>(acc);
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == nstages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    wgmma_wait<0>();
+    fence_regs<BN / 2>(acc);
+    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+    // =========================== epilogue (the producer already loads the next tile) ===========================
+    store_rows<BN>(p, acc, c, cw * 64, alpha);
   }
 }
 
@@ -360,15 +528,16 @@ int encode_tmap(CUtensorMap* out, const TmapSpec& s, bool f32 = false) {
   return 0;
 }
 
-template <bool A_MN, bool B_MN, int BN>
-int launch_impl(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmBlo, int b_split,
-                const CUtensorMap& tmAlo, int a_split, const GemmParams& p, dim3 grid, size_t smem, cudaStream_t stream) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<A_MN, B_MN, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         SMEM_LIMIT);
+using GemmKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, GemmParams);
+
+// majors (profile record): bit 1 = MN-major A, bit 0 = MN-major B, bit 2 = persistent kernel
+int launch_impl(GemmKernel k, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmBlo,
+                const CUtensorMap& tmAlo, const GemmParams& p, int majors, dim3 grid, size_t smem, cudaStream_t stream) {
+  static std::set<GemmKernel> attr_set;
+  if (attr_set.count(k) == 0) {
+    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
     if (e != cudaSuccess) return static_cast<int>(e);
-    attr_set = true;
+    attr_set.insert(k);
   }
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   if (g_profile) {
@@ -376,29 +545,51 @@ int launch_impl(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMa
     cudaEventCreate(&e1);
     cudaEventRecord(e0, stream);
   }
-  gemm_tc_kernel<A_MN, B_MN, BN><<<grid, NUM_THREADS, smem, stream>>>(tmA, tmB, tmBlo, b_split, tmAlo, a_split, p);
+  k<<<grid, NUM_THREADS, smem, stream>>>(tmA, tmB, tmBlo, tmAlo, p);
   if (g_profile) {
     cudaEventRecord(e1, stream);
     g_profile_events.emplace_back(e0, e1);
     g_profile_params.push_back(p);
-    g_profile_majors.push_back((A_MN ? 2 : 0) | (B_MN ? 1 : 0));
+    g_profile_majors.push_back(majors);
   }
   ++g_launch_count;
   return static_cast<int>(cudaGetLastError());
 }
 
-template <bool A_MN, bool B_MN>
-int launch_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmBlo, int b_split,
-              const CUtensorMap& tmAlo, int a_split, const GemmParams& p, dim3 grid, size_t smem, cudaStream_t stream) {
-  switch (p.block_n) {
-    case 16: return launch_impl<A_MN, B_MN, 16>(tmA, tmB, tmBlo, b_split, tmAlo, a_split, p, grid, smem, stream);
-    case 32: return launch_impl<A_MN, B_MN, 32>(tmA, tmB, tmBlo, b_split, tmAlo, a_split, p, grid, smem, stream);
-    case 48: return launch_impl<A_MN, B_MN, 48>(tmA, tmB, tmBlo, b_split, tmAlo, a_split, p, grid, smem, stream);
-    case 64: return launch_impl<A_MN, B_MN, 64>(tmA, tmB, tmBlo, b_split, tmAlo, a_split, p, grid, smem, stream);
-    case 96: return launch_impl<A_MN, B_MN, 96>(tmA, tmB, tmBlo, b_split, tmAlo, a_split, p, grid, smem, stream);
-    case 128: return launch_impl<A_MN, B_MN, 128>(tmA, tmB, tmBlo, b_split, tmAlo, a_split, p, grid, smem, stream);
-    case 192: return launch_impl<A_MN, B_MN, 192>(tmA, tmB, tmBlo, b_split, tmAlo, a_split, p, grid, smem, stream);
-    default: return launch_impl<A_MN, B_MN, 256>(tmA, tmB, tmBlo, b_split, tmAlo, a_split, p, grid, smem, stream);
+// Kernel instance of (A_MN, B_MN, tile width, planes); nullptr for a combination the engine never launches.
+template <bool B_MN, int BN>
+GemmKernel persistent_kernel(int planes) {
+  switch (planes) {
+    case 0: return gemm_persistent_kernel<B_MN, BN, 0>;
+    case PL_BLO: return gemm_persistent_kernel<B_MN, BN, PL_BLO>;
+    case PL_ALO: return gemm_persistent_kernel<B_MN, BN, PL_ALO>;
+    default: return gemm_persistent_kernel<B_MN, BN, PL_BLO | PL_ALO>;
+  }
+}
+template <bool B_MN>
+GemmKernel pick_kernel(bool persistent, int bn, int planes) {
+  if (persistent) {
+    switch (bn) {
+      case 16: return persistent_kernel<B_MN, 16>(planes);
+      case 32: return persistent_kernel<B_MN, 32>(planes);
+      case 48: return persistent_kernel<B_MN, 48>(planes);
+      case 64: return persistent_kernel<B_MN, 64>(planes);
+      case 96: return persistent_kernel<B_MN, 96>(planes);
+      case 128: return persistent_kernel<B_MN, 128>(planes);
+      case 192: return persistent_kernel<B_MN, 192>(planes);
+      default: return persistent_kernel<B_MN, 256>(planes);
+    }
+  }
+  if (planes != 0) return nullptr;  // MN-major A (weight gradients) carries no lo planes
+  switch (bn) {
+    case 16: return gemm_tc_kernel<B_MN, 16>;
+    case 32: return gemm_tc_kernel<B_MN, 32>;
+    case 48: return gemm_tc_kernel<B_MN, 48>;
+    case 64: return gemm_tc_kernel<B_MN, 64>;
+    case 96: return gemm_tc_kernel<B_MN, 96>;
+    case 128: return gemm_tc_kernel<B_MN, 128>;
+    case 192: return gemm_tc_kernel<B_MN, 192>;
+    default: return gemm_tc_kernel<B_MN, 256>;
   }
 }
 
@@ -453,6 +644,7 @@ int launch_gemm(const TmapSpec& A, const TmapSpec& Bin, int a_mn, int b_mn, cons
   if (p.kind != GEMM_CONV_WGRAD || p.kfactor < 1) p.kfactor = 1;
   const int kf = p.kfactor;
   if (kf > 1 && (!a_mn || !b_mn || p.PW * p.PH != 64 * kf || kf > 4)) return -15;
+  if (p.kind == GEMM_CONV_WGRAD && !a_mn) return -15;  // dY patches are MN-major
   int m_tiles;
   if (p.kind == GEMM_CONV) {
     m_tiles = p.nimg * p.tiles_h * p.tiles_w;
@@ -472,18 +664,33 @@ int launch_gemm(const TmapSpec& A, const TmapSpec& Bin, int a_mn, int b_mn, cons
   if (stages < 1) return -13;
   p.num_stages = stages;
   const size_t smem = static_cast<size_t>(stages) * stage_bytes + 1024;
-
-  dim3 grid(m_tiles, n_tiles, p.nz1 * p.nz2 * p.nsplit);
-  if (grid.y > 65535 || grid.z > 65535) return -14;
   p.epi_tma = 0;
   p.epi_op = 0;
   p.cluster = 1;
   p.pair = 0;
 
-  if (!a_mn && !b_mn) return launch_bn<false, false>(tmA, tmB, tmBlo, b_split, tmAlo, a_split, p, grid, smem, stream);
-  if (!a_mn && b_mn) return launch_bn<false, true>(tmA, tmB, tmBlo, b_split, tmAlo, a_split, p, grid, smem, stream);
-  if (a_mn && b_mn) return launch_bn<true, true>(tmA, tmB, tmBlo, b_split, tmAlo, a_split, p, grid, smem, stream);
-  return launch_bn<true, false>(tmA, tmB, tmBlo, b_split, tmAlo, a_split, p, grid, smem, stream);
+  // The weight products (K-major A: linears, 1x1 and 3x3 convs forward and data gradient) run persistent; weight
+  // gradients (MN-major A: split-K with fp32 atomics, 3x3 wgrad with tall stages) keep one tile per CTA.
+  const bool persistent = !a_mn;
+  const int planes = (b_split ? PL_BLO : 0) | (a_split ? PL_ALO : 0);
+  GemmKernel k = b_mn ? pick_kernel<true>(persistent, p.block_n, planes) : pick_kernel<false>(persistent, p.block_n, planes);
+  if (k == nullptr) return -17;
+  const int majors = (a_mn ? 2 : 0) | (b_mn ? 1 : 0) | (persistent ? 4 : 0);
+  const long long tiles = static_cast<long long>(m_tiles) * n_tiles * p.nz1 * p.nz2 * p.nsplit;
+  if (persistent) {
+    if (tiles > INT_MAX) return -14;
+    static const int num_sms = [] {
+      int dev = 0, n = 0;
+      cudaGetDevice(&dev);
+      cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+      return n;
+    }();
+    const long long ctas = std::min<long long>(tiles, std::max(1, num_sms - g_sm_reserve));
+    return launch_impl(k, tmA, tmB, tmBlo, tmAlo, p, majors, dim3(static_cast<unsigned>(ctas)), smem, stream);
+  }
+  dim3 grid(m_tiles, n_tiles, p.nz1 * p.nz2 * p.nsplit);
+  if (grid.y > 65535 || grid.z > 65535) return -14;
+  return launch_impl(k, tmA, tmB, tmBlo, tmAlo, p, majors, grid, smem, stream);
 }
 
 }  // namespace mdm

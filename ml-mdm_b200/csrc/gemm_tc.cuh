@@ -43,7 +43,7 @@ int launch_gemm(const TmapSpec& A, const TmapSpec& B, int a_mn, int b_mn, const 
 
 // Counts kernel launches issued by this library (bench.py reports it as gpu_launches).
 extern unsigned long long g_launch_count;
-extern int g_sm_reserve;  // mdm_set_sm_reserve; the one-tile-per-CTA kernel leaves SMs free between tiles anyway
+extern int g_sm_reserve;  // mdm_set_sm_reserve: SMs the persistent GEMM grid leaves free for collectives
 extern bool g_profile;
 extern std::vector<std::pair<cudaEvent_t, cudaEvent_t>> g_profile_events;
 extern std::vector<mdm_gemm_params> g_profile_params;
