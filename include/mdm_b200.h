@@ -82,7 +82,8 @@ typedef struct mdm_gemm_params {
                     * (<= 64 channels) move only 4-8 KB per 64-pixel stage, so the stage round trip, not HBM, sets
                     * the pace; 256-pixel stages cut the round trips four-fold. Needs a PW x PH = 64 * kfactor patch. */
   int32_t pair;   /* reserved (the launcher sets 0) */
-  int32_t epi_op; /* reserved (the launcher sets 0) */
+  int32_t epi_op; /* filled by the launcher: 1 = the persistent kernel's epilogue runs from a shared-memory staging
+                   * tile on warps of its own, overlapped with the next tile's MMAs; 0 = from the accumulator registers */
 } mdm_gemm_params;
 
 /* Measurement aid for bench.py's roofline leg: while enabled every launch of the wgmma GEMM kernel

@@ -36,7 +36,8 @@ constexpr int SLAB_BYTES = 64 * 64 * 2;  // one 64(k) x 64(mn) MN-major slab
 constexpr int MAX_STAGES = 8;
 constexpr int SMEM_LIMIT = 226 * 1024;  // dynamic shared memory; with the static barriers within H100's 227 KB a block
 
-// warpgroup 0: TMA producer (one thread); warpgroups 1 and 2: wgmma consumers, 64 tile rows each, and the epilogue
+// warpgroup 0: TMA producer (one thread) and, staged, the epilogue warps (1-3); warpgroups 1 and 2: wgmma consumers, 64
+// tile rows each, and the in-register epilogue
 constexpr int NUM_THREADS = 384;
 constexpr int RASTER_N = 8;   // column tiles per band of the persistent kernel's tile order
 
@@ -242,6 +243,144 @@ __device__ __forceinline__ float epi_alpha(const GemmParams& p) {
   return p.alpha_dev != nullptr ? p.alpha * __ldg(p.alpha_dev) : p.alpha;
 }
 
+// Staged epilogue of the persistent kernel: the consumers park their raw accumulators in a shared-memory tile and go
+// on to the next tile's MMAs while warps 1-3 of warpgroup 0 (idle otherwise: one thread issues the TMA loads) run the
+// epilogue from there.
+constexpr int EPI_THREADS = 96;
+constexpr int EPI_ROWS = 8;  // rows each epilogue thread has in flight: 96 x 8 x 16 B = 12 KB of residual loads per SM
+// Row stride of the staging tile: BN + STAGE_PAD floats. The pad spreads a half-warp's float2 fragment stores over all
+// 32 banks (a 512 B row stride would put them 8-way on the same banks).
+constexpr int STAGE_PAD = 8;
+
+// Raw accumulators of 64 tile rows (r0 .. r0 + 63) of one m64 wgmma into the staging tile.
+template <int BN>
+__device__ __forceinline__ void stage_rows(float* stg, const float* acc, int r0) {
+  const int lane = threadIdx.x & 31;
+  const int wq = (threadIdx.x >> 5) & 3;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float* row = stg + (r0 + wq * 16 + (lane >> 2) + 8 * h) * (BN + STAGE_PAD) + (lane & 3) * 2;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+      *reinterpret_cast<float2*>(row + j * 8) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+  }
+}
+
+// Epilogue of one staged tile by epilogue thread et (0 .. 95). Each thread owns one quad of 4 adjacent columns (96 is
+// a multiple of every BN / 4) and walks the tile's rows, so a warp's loads and stores cover whole row segments and the
+// bias is read once per tile. The arithmetic is epi_pair's, operation by operation (alpha, bias, residual, then the
+// stores); the explicitly rounded mul / adds keep v * alpha + bias unfused, as epi_pair compiles. The launcher keeps
+// GELU and GELU' epilogues on the in-register path, so there are none here (out_act_f16 receives a copy of out_f16).
+// vec: every output / operand row is 16 B (fp32) or 8 B (fp16) aligned at each column quad.
+template <int BN>
+__device__ __forceinline__ void epilogue_staged(const GemmParams& p, const float* stg, const TileCoord& c, int et,
+                                                float alpha, bool vec) {
+  constexpr int QPR = BN / 4;            // column quads per row
+  constexpr int RPP = EPI_THREADS / QPR;  // rows per pass of the 96 threads
+  const int q = et % QPR;
+  const int col0 = c.n0 + 4 * q;
+  if (col0 >= p.N) return;
+  const int ncol = min(4, p.N - col0);
+  const bool full = vec && ncol == 4;
+  float bias[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) bias[e] = (p.bias != nullptr && e < ncol) ? __ldg(p.bias + col0 + e) : 0.f;
+  __half* o16[2] = {reinterpret_cast<__half*>(p.out_f16), reinterpret_cast<__half*>(p.out_act_f16)};
+
+  for (int rb = et / QPR; rb < BLOCK_M; rb += RPP * EPI_ROWS) {
+    long long off[EPI_ROWS];
+    float v[EPI_ROWS][4];
+    // output offsets (-1: row outside the output) and the staged accumulators
+#pragma unroll
+    for (int u = 0; u < EPI_ROWS; ++u) {
+      const int r = rb + u * RPP;
+      off[u] = -1;
+      if (r < BLOCK_M) {
+        const float4 a = *reinterpret_cast<const float4*>(stg + r * (BN + STAGE_PAD) + 4 * q);
+        v[u][0] = a.x;
+        v[u][1] = a.y;
+        v[u][2] = a.z;
+        v[u][3] = a.w;
+        if (p.kind == GEMM_CONV) {
+          const int ph = r / p.PW;
+          const int pw = r - ph * p.PW;
+          const int hh = c.th * p.PH + ph;
+          const int ww = c.tw * p.PW + pw;
+          if (hh < p.H && ww < p.W && c.img < p.nimg)
+            off[u] = (static_cast<long long>(c.img * p.H + hh) * p.W + ww) * p.ldc + col0;
+        } else if (c.m0 + r < p.M) {
+          off[u] = static_cast<long long>(c.m0 + r) * p.ldc + static_cast<long long>(c.z1) * p.c_z1_stride +
+                   static_cast<long long>(c.z2) * p.c_z2_stride + col0;
+        }
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < EPI_ROWS; ++u)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) v[u][e] = __fmul_rn(v[u][e], alpha);
+    if (p.bias != nullptr) {
+#pragma unroll
+      for (int u = 0; u < EPI_ROWS; ++u)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) v[u][e] = __fadd_rn(v[u][e], bias[e]);
+    }
+    if (p.residual != nullptr) {
+      // all rows' loads first, so EPI_ROWS of them are in flight
+      float res[EPI_ROWS][4];
+#pragma unroll
+      for (int u = 0; u < EPI_ROWS; ++u) {
+        if (off[u] < 0) continue;
+        if (full) {
+          const float4 x = __ldg(reinterpret_cast<const float4*>(p.residual + off[u]));
+          res[u][0] = x.x;
+          res[u][1] = x.y;
+          res[u][2] = x.z;
+          res[u][3] = x.w;
+        } else {
+#pragma unroll
+          for (int e = 0; e < 4; ++e) res[u][e] = e < ncol ? __ldg(p.residual + off[u] + e) : 0.f;
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < EPI_ROWS; ++u)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) v[u][e] = __fadd_rn(v[u][e], res[u][e]);
+    }
+#pragma unroll
+    for (int u = 0; u < EPI_ROWS; ++u) {
+      if (off[u] < 0) continue;
+      if (p.out_f32 != nullptr) {
+        float* o = p.out_f32 + off[u];
+        if (full) {
+          *reinterpret_cast<float4*>(o) = make_float4(v[u][0], v[u][1], v[u][2], v[u][3]);
+        } else {
+#pragma unroll
+          for (int e = 0; e < 4; ++e)
+            if (e < ncol) o[e] = v[u][e];
+        }
+      }
+#pragma unroll
+      for (int t = 0; t < 2; ++t) {
+        if (o16[t] == nullptr) continue;
+        const float* a = v[u];
+        __half* o = o16[t] + off[u];
+        if (full) {
+          const __half2 h01 = __floats2half2_rn(a[0], a[1]);
+          const __half2 h23 = __floats2half2_rn(a[2], a[3]);
+          uint2 x;
+          x.x = *reinterpret_cast<const uint32_t*>(&h01);
+          x.y = *reinterpret_cast<const uint32_t*>(&h23);
+          *reinterpret_cast<uint2*>(o) = x;
+        } else {
+#pragma unroll
+          for (int e = 0; e < 4; ++e)
+            if (e < ncol) o[e] = __float2half_rn(a[e]);
+        }
+      }
+    }
+  }
+}
+
 // One output tile per CTA: the weight gradients (MN-major A: plain MN x MN with split-K, 3x3 wgrad with tall stages).
 template <bool B_MN, int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
@@ -369,12 +508,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   store_rows<BN>(p, acc, c, cw * 64, epi_alpha(p));
 }
 
-// Persistent schedule of the weight products (plain K x K, plain K x MN, 3x3 conv forward / data gradient; K-major A,
-// BN <= 128). Each CTA walks tiles blockIdx.x + i * gridDim.x in the order of the one-tile grid, and the producer
-// streams the k blocks of all its tiles through one stage ring, so the next tile's stages load while the consumers
-// run the epilogue of the last one. Both consumer warpgroups work on every tile, 64 rows each, as in the one-tile
-// kernel. (Consumers taking alternate whole tiles, one in its epilogue while the other issues MMAs, measured slower:
-// at 128 accumulators per thread the epilogue of a whole tile on one warpgroup took more than twice as long.)
+// Persistent schedule of the weight products (plain K x K, plain K x MN, 3x3 conv forward / data gradient; K-major A).
+// Each CTA walks tiles blockIdx.x + i * gridDim.x, and the producer streams the k blocks of all its tiles through one
+// stage ring, so the next tile's stages load while the last one is drained. Both consumer warpgroups work on every
+// tile, 64 rows each, as in the one-tile kernel. (Consumers taking alternate whole tiles, one in its epilogue while
+// the other issues MMAs, measured slower: at 128 accumulators per thread the epilogue of a whole tile on one
+// warpgroup took more than twice as long.)
+// p.epi_op = 1 (staged epilogue, BN <= 128): after a tile's last MMA the consumers wait until the staging tile behind
+// the stage ring is free, store their raw accumulators there, arrive on staged_full and start the next tile; warps 1-3
+// of warpgroup 0 walk the same tile sequence, run each tile's epilogue from the staging tile and arrive on
+// staged_free. The epilogue then overlaps the next tile's MMAs instead of holding up the tensor cores.
+// p.epi_op = 0: the consumers run the epilogue from their registers after the mainloop.
 template <bool B_MN, int BN, int PL>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -383,11 +527,13 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[MAX_STAGES];
   __shared__ __align__(8) uint64_t empty_bar[MAX_STAGES];
+  __shared__ __align__(8) uint64_t staged_full, staged_free;
 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   const int wg = threadIdx.x >> 7;
   using S = StageLayout<B_MN, BN, PL>;
+  const bool staged = BN <= 128 && p.epi_op == 1;
   const int nstages = p.num_stages;
   const int m_tiles = p.kind == GEMM_CONV ? p.nimg * p.tiles_h * p.tiles_w : (p.M + BLOCK_M - 1) / BLOCK_M;
   const int n_tiles = (p.N + BN - 1) / BN;
@@ -414,14 +560,16 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 8);  // one arrival per consumer warp
     }
+    mbar_init(&staged_full, 256);  // every consumer thread
+    mbar_init(&staged_free, EPI_THREADS);
     fence_barrier_init();
   }
   __syncthreads();
+  float* stg = reinterpret_cast<float*>(smem + nstages * S::bytes);
 
   if (wg == 0) {
     // =========================== TMA producer ===========================
-    reg_dealloc<40>();
-    if (threadIdx.x == 0) {
+    auto produce = [&] {
       int stage = 0;
       uint32_t phase = 0;
       for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
@@ -439,18 +587,47 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
           }
         }
       }
+    };
+    // (each branch keeps its own register budget: code after a join would be compiled for the smaller one)
+    if (!staged) {
+      reg_dealloc<40>();
+      if (threadIdx.x == 0) produce();
+    } else if constexpr (BN <= 128) {
+      reg_dealloc<152>();
+      if (threadIdx.x == 0) {
+        produce();
+      } else if (threadIdx.x >= 32) {
+        // =========================== epilogue warps (staged) ===========================
+        const float alpha = epi_alpha(p);
+        const bool vec = ((p.ldc | p.c_z1_stride | p.c_z2_stride) & 3) == 0 &&
+                         ((reinterpret_cast<uintptr_t>(p.out_f32) | reinterpret_cast<uintptr_t>(p.residual)) & 15) == 0 &&
+                         ((reinterpret_cast<uintptr_t>(p.out_f16) | reinterpret_cast<uintptr_t>(p.out_act_f16)) & 7) == 0;
+        uint32_t sphase = 0;
+        for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+          const TileCoord c = coord(t);
+          mbar_wait(&staged_full, sphase);
+          epilogue_staged<BN>(p, stg, c, threadIdx.x - 32, alpha, vec);
+          mbar_arrive(&staged_free);
+          sphase ^= 1;
+        }
+      }
     }
     return;
   }
 
   // =========================== wgmma consumers ===========================
-  reg_alloc<232>();
+  if (staged) {
+    reg_alloc<168>();
+  } else {
+    reg_alloc<232>();
+  }
   const int cw = wg - 1;  // this warpgroup's 64 rows of every tile
   const int lane = threadIdx.x & 31;
   const float alpha = epi_alpha(p);
   float acc[BN / 2];
   int stage = 0;
   uint32_t phase = 0;
+  uint32_t sphase = 0;
   for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
     const TileCoord c = coord(t);
     int prev = -1;
@@ -478,6 +655,15 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     wgmma_wait<0>();
     fence_regs<BN / 2>(acc);
     if (lane == 0) mbar_arrive(&empty_bar[prev]);
+    if constexpr (BN <= 128) {
+      if (staged) {
+        mbar_wait(&staged_free, sphase ^ 1);  // the epilogue warps are done with the previous tile
+        stage_rows<BN>(stg, acc, cw * 64);
+        mbar_arrive(&staged_full);
+        sphase ^= 1;
+        continue;
+      }
+    }
     // =========================== epilogue (the producer already loads the next tile) ===========================
     store_rows<BN>(p, acc, c, cw * 64, alpha);
   }
@@ -656,22 +842,33 @@ int launch_gemm(const TmapSpec& A, const TmapSpec& Bin, int a_mn, int b_mn, cons
   const int nb_alloc = b_mn ? ((p.block_n + 63) / 64) * 64 : p.block_n;
   const int stage_bytes =
       kf > 1 ? ((p.M <= 64 ? 1 : 2) + nb_alloc / 64) * SLAB_BYTES * kf : A_STAGE_BYTES * (1 + a_split) + nb_alloc * 128 * (1 + b_split);
-  // one CTA per SM (384 threads at the consumers' register budget): the whole shared memory goes to the pipeline
-  int stages = (SMEM_LIMIT - 1024) / stage_bytes;
-  if (stages > MAX_STAGES) stages = MAX_STAGES;
+  // one CTA per SM (384 threads at the consumers' register budget): the whole shared memory goes to the pipeline,
+  // less the staging tile of a staged epilogue
   const int per = (p.num_kblocks + p.nsplit - 1) / p.nsplit;
-  if (stages > per) stages = per;
+  auto ring = [&](int reserved) { return std::min({(SMEM_LIMIT - 1024 - reserved) / stage_bytes, MAX_STAGES, per}); };
+  int stages = ring(0);
   if (stages < 1) return -13;
-  p.num_stages = stages;
-  const size_t smem = static_cast<size_t>(stages) * stage_bytes + 1024;
-  p.epi_tma = 0;
-  p.epi_op = 0;
-  p.cluster = 1;
-  p.pair = 0;
 
   // The weight products (K-major A: linears, 1x1 and 3x3 convs forward and data gradient) run persistent; weight
   // gradients (MN-major A: split-K with fp32 atomics, 3x3 wgrad with tall stages) keep one tile per CTA.
   const bool persistent = !a_mn;
+  // Staged epilogue (gemm_persistent_kernel) for tiles up to 128 columns, where the staging tile still leaves a ring
+  // of three stages (or every k block of a short contraction): with two, the producer can no longer load a stage ahead
+  // of the two the consumers hold, and the MMAs wait on TMA. Epilogues that evaluate the erf-GELU or its derivative
+  // per element keep the in-register path: on three warps that arithmetic outlasts the next tile's mainloop (the FFN
+  // up-projection and its data gradient ran up to 32 % slower staged on an H100). Split-K atomics keep it too.
+  const int staging = BLOCK_M * (p.block_n + STAGE_PAD) * 4;
+  const bool gelu_math = (p.act == ACT_GELU && p.out_act_f16 != nullptr) || p.gelu_grad_src != nullptr;
+  const bool staged =
+      persistent && p.block_n <= 128 && !p.atomic && !gelu_math && ring(staging) >= std::min(3, per);
+  if (staged) stages = ring(staging);
+  p.num_stages = stages;
+  const size_t smem = static_cast<size_t>(stages) * stage_bytes + 1024 + (staged ? staging : 0);
+  p.epi_tma = 0;
+  p.epi_op = staged ? 1 : 0;
+  p.cluster = 1;
+  p.pair = 0;
+
   const int planes = (b_split ? PL_BLO : 0) | (a_split ? PL_ALO : 0);
   GemmKernel k = b_mn ? pick_kernel<true>(persistent, p.block_n, planes) : pick_kernel<false>(persistent, p.block_n, planes);
   if (k == nullptr) return -17;

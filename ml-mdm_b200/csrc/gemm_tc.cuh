@@ -10,8 +10,8 @@
 //
 // Operands are fp16 in HBM, staged by TMA into 128B-swizzled shared memory through an mbarrier pipeline, multiplied
 // by wgmma (two consumer warpgroups of 64 x N x 16 instructions, N <= 256) with fp32 accumulators in registers, and
-// drained straight from registers by a fused epilogue (alpha, bias, residual add, GELU, fp32/fp16 stores, split-K
-// atomics).
+// drained by a fused epilogue (alpha, bias, residual add, GELU, fp32/fp16 stores, split-K atomics), from the registers
+// or, in the persistent kernel, from a shared-memory staging tile on warps of its own.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
