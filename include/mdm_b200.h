@@ -75,7 +75,13 @@ typedef struct mdm_gemm_params {
   int64_t ldc, c_z1_stride, c_z2_stride;
   int32_t act;
   int32_t atomic;
-  int32_t epi_tma; /* reserved (the launcher sets 0): the epilogue stores straight from the accumulator registers */
+  int32_t epi_tma; /* filled by the launcher: 1 = TMA epilogue (with epi_op = 1): the residual or GELU' source is loaded
+                    * by TMA into the staging tile while the tile's MMAs run, the consumers fold their accumulators into
+                    * it, and the outputs are written by TMA stores. Chosen for plain products with a GELU or GELU'
+                    * epilogue or at most 8 k blocks, where tensor maps can describe every epilogue buffer: 16 B-aligned
+                    * bases, ldc and batch strides multiples of 16 B, a tile width that is a multiple of 32 columns up
+                    * to 128, fp32 buffers (residual, out_f32) or fp16 ones (GELU' source, out_f16, out_act_f16) but
+                    * not both, no split-K atomics. 0 = the epilogue loads and stores with ordinary instructions */
   const void* gelu_grad_src; /* optional __half*, indexed like the output: result *= gelu'(src) (FFN backward) */
   int32_t cluster; /* reserved (the launcher sets 1): every CTA loads its own B tile */
   int32_t kfactor; /* MDM_GEMM_CONV_WGRAD only: pixel rows per pipeline stage = 64 * kfactor (0/1: 64). Narrow layers

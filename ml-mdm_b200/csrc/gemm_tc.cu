@@ -6,6 +6,7 @@
 
 #include <algorithm>
 #include <climits>
+#include <cstring>
 #include <set>
 #include <utility>
 #include <vector>
@@ -381,12 +382,130 @@ __device__ __forceinline__ void epilogue_staged(const GemmParams& p, const float
   }
 }
 
+// TMA epilogue of the persistent kernel (p.epi_tma = 1). The staging tile is a row of 128-row panels, 32 columns each,
+// in the 128B (fp32) or 64B (fp16) swizzle of a 32-column TMA box, so one box loads or stores a whole panel and the
+// consumers' fragment accesses stay free of bank conflicts. An epilogue touches fp32 planes (residual, out_f32) or fp16
+// ones (GELU' source, out_f16, out_act_f16), never both (the launcher's rule): the fp32 plane fills the staging tile;
+// fp16 plane 0 (GELU' source, then out_f16) its first half and fp16 plane 1 (out_act_f16) its second.
+// Plain mode only (see epi_tma_maps): the tensor maps view each epilogue buffer as (N, M, z1, z2).
+struct EpiMaps {
+  CUtensorMap src;   // residual (fp32) or GELU' source (fp16)
+  CUtensorMap o32;   // out_f32
+  CUtensorMap o16;   // out_f16
+  CUtensorMap oact;  // out_act_f16
+};
+constexpr int EPI_PANEL = 32;                       // columns per panel
+constexpr int EPI_PANEL_F32 = BLOCK_M * EPI_PANEL * 4;  // bytes of one fp32 panel
+constexpr int EPI_PANEL_F16 = BLOCK_M * EPI_PANEL * 2;
+
+// byte offsets of element (r, c) of the staging tile, c even (the pair c, c + 1 is contiguous)
+__device__ __forceinline__ uint32_t epi_off_f32(int r, int c) {
+  const int cc = c & 31;
+  return (c >> 5) * EPI_PANEL_F32 + r * 128 + ((((cc >> 2) ^ r) & 7) << 4) + (cc & 3) * 4;
+}
+template <int BN>
+__device__ __forceinline__ uint32_t epi_off_f16(int plane, int r, int c) {
+  const int cc = c & 31;
+  return plane * (BN / EPI_PANEL) * EPI_PANEL_F16 + (c >> 5) * EPI_PANEL_F16 + r * 64 +
+         ((((cc >> 3) ^ (r >> 1)) & 3) << 4) + (cc & 7) * 2;
+}
+
+// The consumers' part of the TMA epilogue for 64 tile rows (r0 .. r0 + 63): epi_pair's arithmetic on the accumulators,
+// operation by operation (explicitly rounded, so v * alpha + bias stays unfused as epi_pair compiles), with the
+// residual or GELU' source read from the staging tile where the epilogue thread's TMA load left it, and the results
+// written back over it for the TMA stores. Every element is read and written by the same thread. Rows and columns
+// outside the output compute on zero fill and are never stored.
+template <int BN>
+__device__ __forceinline__ void fold_rows(const GemmParams& p, uint8_t* stg, const float* acc, int n0, int r0,
+                                          float alpha) {
+  const int lane = threadIdx.x & 31;
+  const int wq = (threadIdx.x >> 5) & 3;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = r0 + wq * 16 + (lane >> 2) + 8 * h;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int c = j * 8 + (lane & 3) * 2;
+      const int col = n0 + c;
+      float v0 = __fmul_rn(acc[4 * j + 2 * h], alpha);
+      float v1 = __fmul_rn(acc[4 * j + 2 * h + 1], alpha);
+      if (p.bias != nullptr) {
+        v0 = __fadd_rn(v0, col < p.N ? __ldg(p.bias + col) : 0.f);
+        v1 = __fadd_rn(v1, col + 1 < p.N ? __ldg(p.bias + col + 1) : 0.f);
+      }
+      float2* s32 = reinterpret_cast<float2*>(stg + epi_off_f32(r, c));
+      __half2* s16 = reinterpret_cast<__half2*>(stg + epi_off_f16<BN>(0, r, c));
+      if (p.residual != nullptr) {
+        const float2 x = *s32;
+        v0 = __fadd_rn(v0, x.x);
+        v1 = __fadd_rn(v1, x.y);
+      }
+      if (p.gelu_grad_src != nullptr) {
+        const float2 x = __half22float2(*s16);
+        v0 = __fmul_rn(v0, gelu_grad(x.x));
+        v1 = __fmul_rn(v1, gelu_grad(x.y));
+      }
+      if (p.out_f32 != nullptr) *s32 = make_float2(v0, v1);
+      if (p.out_f16 != nullptr) *s16 = __floats2half2_rn(v0, v1);
+      if (p.out_act_f16 != nullptr) {
+        const bool g = p.act == ACT_GELU;
+        *reinterpret_cast<__half2*>(stg + epi_off_f16<BN>(1, r, c)) =
+            __floats2half2_rn(g ? gelu_erf(v0) : v0, g ? gelu_erf(v1) : v1);
+      }
+    }
+  }
+}
+
+// TMA coordinates of panel j of a tile (see EpiMaps)
+__device__ __forceinline__ void epi_coords(const TileCoord& c, int j, int* x) {
+  x[0] = c.n0 + j * EPI_PANEL;
+  x[1] = c.m0;
+  x[2] = c.z1;
+  x[3] = c.z2;
+}
+
+// The epilogue thread's TMA load of a tile's residual / GELU' source into the staging tile, completing on bar (which
+// it arrives on, with or without a source).
+template <int BN>
+__device__ __forceinline__ void epi_load_source(const GemmParams& p, const EpiMaps& em, uint8_t* stg, uint64_t* bar,
+                                                const TileCoord& c) {
+  const bool f32 = p.residual != nullptr;
+  if (!f32 && p.gelu_grad_src == nullptr) {
+    mbar_arrive(bar);
+    return;
+  }
+  const int panel = f32 ? EPI_PANEL_F32 : EPI_PANEL_F16;
+  mbar_expect_tx(bar, static_cast<uint32_t>((BN / EPI_PANEL) * panel));
+#pragma unroll
+  for (int j = 0; j < BN / EPI_PANEL; ++j) {
+    int x[4];
+    epi_coords(c, j, x);
+    tma_load_4d(stg + j * panel, &em.src, bar, x[0], x[1], x[2], x[3]);
+  }
+}
+
+// The epilogue thread's TMA stores of a folded tile.
+template <int BN>
+__device__ __forceinline__ void epi_store_tile(const GemmParams& p, const EpiMaps& em, const uint8_t* stg,
+                                               const TileCoord& c) {
+#pragma unroll
+  for (int j = 0; j < BN / EPI_PANEL; ++j) {
+    int x[4];
+    epi_coords(c, j, x);
+    if (p.out_f32 != nullptr) tma_store_4d(&em.o32, stg + j * EPI_PANEL_F32, x[0], x[1], x[2], x[3]);
+    if (p.out_f16 != nullptr) tma_store_4d(&em.o16, stg + j * EPI_PANEL_F16, x[0], x[1], x[2], x[3]);
+    if (p.out_act_f16 != nullptr)
+      tma_store_4d(&em.oact, stg + ((BN / EPI_PANEL) + j) * EPI_PANEL_F16, x[0], x[1], x[2], x[3]);
+  }
+  bulk_commit();
+}
+
 // One output tile per CTA: the weight gradients (MN-major A: plain MN x MN with split-K, 3x3 wgrad with tall stages).
 template <bool B_MN, int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmBlo, const __grid_constant__ CUtensorMap tmAlo,
-               const GemmParams p) {
+               const __grid_constant__ EpiMaps em, const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[MAX_STAGES];
   __shared__ __align__(8) uint64_t empty_bar[MAX_STAGES];
@@ -518,12 +637,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 // the stage ring is free, store their raw accumulators there, arrive on staged_full and start the next tile; warps 1-3
 // of warpgroup 0 walk the same tile sequence, run each tile's epilogue from the staging tile and arrive on
 // staged_free. The epilogue then overlaps the next tile's MMAs instead of holding up the tensor cores.
+// p.epi_tma = 1 (with p.epi_op = 1): the TMA epilogue (see EpiMaps): one epilogue thread loads each tile's residual /
+// GELU' source into the staging tile during its MMAs and stores the consumers' results from there by TMA.
 // p.epi_op = 0: the consumers run the epilogue from their registers after the mainloop.
 template <bool B_MN, int BN, int PL>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                        const __grid_constant__ CUtensorMap tmBlo, const __grid_constant__ CUtensorMap tmAlo,
-                       const GemmParams p) {
+                       const __grid_constant__ EpiMaps em, const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[MAX_STAGES];
   __shared__ __align__(8) uint64_t empty_bar[MAX_STAGES];
@@ -534,6 +655,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   const int wg = threadIdx.x >> 7;
   using S = StageLayout<B_MN, BN, PL>;
   const bool staged = BN <= 128 && p.epi_op == 1;
+  const bool tma_epi = staged && p.epi_tma == 1 && BN % EPI_PANEL == 0;
   const int nstages = p.num_stages;
   const int m_tiles = p.kind == GEMM_CONV ? p.nimg * p.tiles_h * p.tiles_w : (p.M + BLOCK_M - 1) / BLOCK_M;
   const int n_tiles = (p.N + BN - 1) / BN;
@@ -561,11 +683,11 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       mbar_init(&empty_bar[s], 8);  // one arrival per consumer warp
     }
     mbar_init(&staged_full, 256);  // every consumer thread
-    mbar_init(&staged_free, EPI_THREADS);
+    mbar_init(&staged_free, tma_epi ? 1 : EPI_THREADS);
     fence_barrier_init();
   }
   __syncthreads();
-  float* stg = reinterpret_cast<float*>(smem + nstages * S::bytes);
+  uint8_t* stg = smem + nstages * S::bytes;
 
   if (wg == 0) {
     // =========================== TMA producer ===========================
@@ -596,6 +718,25 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       reg_dealloc<152>();
       if (threadIdx.x == 0) {
         produce();
+      } else if (tma_epi) {
+        // =========================== epilogue thread (TMA) ===========================
+        // Phase i of staged_free completes when tile i's source is in the staging tile (at once without a source) and
+        // the stores of tile i - 1 have read it; tile i + 1's source load is issued as soon as tile i's stores have
+        // read the staging tile, so it lands while the consumers run tile i + 1's MMAs.
+        if (threadIdx.x == 32) {
+          if (p.residual != nullptr || p.gelu_grad_src != nullptr) prefetch_tmap(&em.src);
+          uint32_t sphase = 0;
+          if (blockIdx.x < num_tiles) epi_load_source<BN>(p, em, stg, &staged_free, coord(blockIdx.x));
+          for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+            mbar_wait(&staged_full, sphase);
+            sphase ^= 1;
+            epi_store_tile<BN>(p, em, stg, coord(t));
+            bulk_wait_read();
+            if (t + static_cast<int>(gridDim.x) < num_tiles)
+              epi_load_source<BN>(p, em, stg, &staged_free, coord(t + gridDim.x));
+          }
+          bulk_wait_all();
+        }
       } else if (threadIdx.x >= 32) {
         // =========================== epilogue warps (staged) ===========================
         const float alpha = epi_alpha(p);
@@ -606,7 +747,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
         for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
           const TileCoord c = coord(t);
           mbar_wait(&staged_full, sphase);
-          epilogue_staged<BN>(p, stg, c, threadIdx.x - 32, alpha, vec);
+          epilogue_staged<BN>(p, reinterpret_cast<const float*>(stg), c, threadIdx.x - 32, alpha, vec);
           mbar_arrive(&staged_free);
           sphase ^= 1;
         }
@@ -656,9 +797,17 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     fence_regs<BN / 2>(acc);
     if (lane == 0) mbar_arrive(&empty_bar[prev]);
     if constexpr (BN <= 128) {
+      if (tma_epi) {
+        mbar_wait(&staged_free, sphase);  // this tile's source has landed, the previous tile's stores have read it
+        fold_rows<BN>(p, stg, acc, c.n0, cw * 64, alpha);
+        fence_proxy_async();  // before the TMA stores read the results
+        mbar_arrive(&staged_full);
+        sphase ^= 1;
+        continue;
+      }
       if (staged) {
         mbar_wait(&staged_free, sphase ^ 1);  // the epilogue warps are done with the previous tile
-        stage_rows<BN>(stg, acc, cw * 64);
+        stage_rows<BN>(reinterpret_cast<float*>(stg), acc, cw * 64);
         mbar_arrive(&staged_full);
         sphase ^= 1;
         continue;
@@ -714,11 +863,68 @@ int encode_tmap(CUtensorMap* out, const TmapSpec& s, bool f32 = false) {
   return 0;
 }
 
-using GemmKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, GemmParams);
+// Tensor map of an epilogue buffer (see EpiMaps): dims / strides (elements) of dims 1-3, a 32-column panel box,
+// zero fill outside the tensor on loads, clipping on stores.
+int encode_epi_map(CUtensorMap* out, const void* ptr, bool f32, const uint64_t* dims, const uint64_t* strides,
+                   const uint32_t* box) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (fn == nullptr) return -1;
+  const int esz = f32 ? 4 : 2;
+  cuuint64_t gdim[4], gstr[3];
+  cuuint32_t bx[4], estr[4] = {1, 1, 1, 1};
+  for (int i = 0; i < 4; ++i) {
+    gdim[i] = dims[i];
+    bx[i] = box[i];
+  }
+  for (int i = 0; i < 3; ++i) gstr[i] = strides[i] * esz;
+  CUresult r = fn(out, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr),
+                  gdim, gstr, bx, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  f32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : -2;
+}
 
-// majors (profile record): bit 1 = MN-major A, bit 0 = MN-major B, bit 2 = persistent kernel
+constexpr int TMA_EPI_MAX_KBLOCKS = 8;  // see launch_gemm
+
+// Whether the TMA epilogue can serve p (tile width already rounded), and if so its tensor maps.
+bool epi_tma_maps(const GemmParams& p, EpiMaps* em) {
+  const bool uses32 = p.residual != nullptr || p.out_f32 != nullptr;
+  const bool uses16 = p.gelu_grad_src != nullptr || p.out_f16 != nullptr || p.out_act_f16 != nullptr;
+  // (3x3 convs have at least nine k blocks and no GELU, so none qualifies: conv64.fwd measured 10 % slower)
+  if (p.kind != GEMM_PLAIN || uses32 == uses16 || p.atomic || p.block_n % EPI_PANEL != 0 || p.block_n > 128)
+    return false;
+  const long long esz = uses32 ? 4 : 2;
+  const void* bufs[] = {p.residual, p.out_f32, p.gelu_grad_src, p.out_f16, p.out_act_f16};
+  for (const void* b : bufs)
+    if ((reinterpret_cast<uintptr_t>(b) & 15) != 0) return false;
+  uint64_t dims[4], str[3];
+  const uint32_t box[4] = {EPI_PANEL, BLOCK_M, 1, 1};
+  if (p.ldc < p.N || p.N < 1 || p.M < 1) return false;
+  // a batch dimension of one is never stepped: any valid stride will do
+  const long long z1 = p.nz1 > 1 ? p.c_z1_stride : p.ldc * p.M;
+  const long long z2 = p.nz2 > 1 ? p.c_z2_stride : z1 * p.nz1;
+  if (z1 <= 0 || z2 <= 0) return false;
+  const long long s[3] = {p.ldc, z1, z2};
+  const long long d[4] = {p.N, p.M, p.nz1, p.nz2};
+  for (int i = 0; i < 4; ++i) dims[i] = static_cast<uint64_t>(d[i]);
+  for (int i = 0; i < 3; ++i) str[i] = static_cast<uint64_t>(s[i]);
+  for (int i = 0; i < 3; ++i)
+    if ((str[i] * esz) % 16 != 0 || str[i] * esz >= (1ull << 40)) return false;
+  const void* src = uses32 ? static_cast<const void*>(p.residual) : p.gelu_grad_src;
+  if (src != nullptr && encode_epi_map(&em->src, src, uses32, dims, str, box) != 0) return false;
+  if (p.out_f32 != nullptr && encode_epi_map(&em->o32, p.out_f32, true, dims, str, box) != 0) return false;
+  if (p.out_f16 != nullptr && encode_epi_map(&em->o16, p.out_f16, false, dims, str, box) != 0) return false;
+  if (p.out_act_f16 != nullptr && encode_epi_map(&em->oact, p.out_act_f16, false, dims, str, box) != 0) return false;
+  return true;
+}
+
+using GemmKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, EpiMaps, GemmParams);
+
+// majors (profile record): bit 1 = MN-major A, bit 0 = MN-major B, bit 2 = persistent kernel, bit 3 = staged epilogue,
+// bit 4 = TMA epilogue
 int launch_impl(GemmKernel k, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmBlo,
-                const CUtensorMap& tmAlo, const GemmParams& p, int majors, dim3 grid, size_t smem, cudaStream_t stream) {
+                const CUtensorMap& tmAlo, const EpiMaps& em, const GemmParams& p, int majors, dim3 grid, size_t smem,
+                cudaStream_t stream) {
   static std::set<GemmKernel> attr_set;
   if (attr_set.count(k) == 0) {
     cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
@@ -731,7 +937,7 @@ int launch_impl(GemmKernel k, const CUtensorMap& tmA, const CUtensorMap& tmB, co
     cudaEventCreate(&e1);
     cudaEventRecord(e0, stream);
   }
-  k<<<grid, NUM_THREADS, smem, stream>>>(tmA, tmB, tmBlo, tmAlo, p);
+  k<<<grid, NUM_THREADS, smem, stream>>>(tmA, tmB, tmBlo, tmAlo, em, p);
   if (g_profile) {
     cudaEventRecord(e1, stream);
     g_profile_events.emplace_back(e0, e1);
@@ -857,14 +1063,26 @@ int launch_gemm(const TmapSpec& A, const TmapSpec& Bin, int a_mn, int b_mn, cons
   // of the two the consumers hold, and the MMAs wait on TMA. Epilogues that evaluate the erf-GELU or its derivative
   // per element keep the in-register path: on three warps that arithmetic outlasts the next tile's mainloop (the FFN
   // up-projection and its data gradient ran up to 32 % slower staged on an H100). Split-K atomics keep it too.
-  const int staging = BLOCK_M * (p.block_n + STAGE_PAD) * 4;
+  // The TMA epilogue (staged, with the residual / GELU' source loaded into the staging tile and the results stored by
+  // TMA; see EpiMaps) where its tensor maps can describe the epilogue buffers, for GELU / GELU' epilogues and for
+  // contractions of at most TMA_EPI_MAX_KBLOCKS k blocks. Measured on an H100 (tests/profile_gemm_epilogue.py): the FFN
+  // up-projection and its GELU' data gradient ran 20-39 % faster, with GELU / GELU' on the consumers; K = 512
+  // products 11-13 % faster; but K >= 768 products without GELU 3-15 % slower than the staged path below (the
+  // consumers' fold does not explain it; the cause is not found), so those keep it. Its unpadded staging tile is
+  // smaller, so it too keeps three stages.
   const bool gelu_math = (p.act == ACT_GELU && p.out_act_f16 != nullptr) || p.gelu_grad_src != nullptr;
+  alignas(64) EpiMaps em;
+  memset(&em, 0, sizeof(em));
+  const int staging_tma = BLOCK_M * p.block_n * 4;
+  const bool tma = persistent && (gelu_math || per <= TMA_EPI_MAX_KBLOCKS) && ring(staging_tma) >= std::min(3, per) &&
+                   epi_tma_maps(p, &em);
+  const int staging = tma ? staging_tma : BLOCK_M * (p.block_n + STAGE_PAD) * 4;
   const bool staged =
-      persistent && p.block_n <= 128 && !p.atomic && !gelu_math && ring(staging) >= std::min(3, per);
+      tma || (persistent && p.block_n <= 128 && !p.atomic && !gelu_math && ring(staging) >= std::min(3, per));
   if (staged) stages = ring(staging);
   p.num_stages = stages;
   const size_t smem = static_cast<size_t>(stages) * stage_bytes + 1024 + (staged ? staging : 0);
-  p.epi_tma = 0;
+  p.epi_tma = tma ? 1 : 0;
   p.epi_op = staged ? 1 : 0;
   p.cluster = 1;
   p.pair = 0;
@@ -872,7 +1090,7 @@ int launch_gemm(const TmapSpec& A, const TmapSpec& Bin, int a_mn, int b_mn, cons
   const int planes = (b_split ? PL_BLO : 0) | (a_split ? PL_ALO : 0);
   GemmKernel k = b_mn ? pick_kernel<true>(persistent, p.block_n, planes) : pick_kernel<false>(persistent, p.block_n, planes);
   if (k == nullptr) return -17;
-  const int majors = (a_mn ? 2 : 0) | (b_mn ? 1 : 0) | (persistent ? 4 : 0);
+  const int majors = (a_mn ? 2 : 0) | (b_mn ? 1 : 0) | (persistent ? 4 : 0) | (staged ? 8 : 0) | (tma ? 16 : 0);
   const long long tiles = static_cast<long long>(m_tiles) * n_tiles * p.nz1 * p.nz2 * p.nsplit;
   if (persistent) {
     if (tiles > INT_MAX) return -14;
@@ -883,11 +1101,11 @@ int launch_gemm(const TmapSpec& A, const TmapSpec& Bin, int a_mn, int b_mn, cons
       return n;
     }();
     const long long ctas = std::min<long long>(tiles, std::max(1, num_sms - g_sm_reserve));
-    return launch_impl(k, tmA, tmB, tmBlo, tmAlo, p, majors, dim3(static_cast<unsigned>(ctas)), smem, stream);
+    return launch_impl(k, tmA, tmB, tmBlo, tmAlo, em, p, majors, dim3(static_cast<unsigned>(ctas)), smem, stream);
   }
   dim3 grid(m_tiles, n_tiles, p.nz1 * p.nz2 * p.nsplit);
   if (grid.y > 65535 || grid.z > 65535) return -14;
-  return launch_impl(k, tmA, tmB, tmBlo, tmAlo, p, majors, grid, smem, stream);
+  return launch_impl(k, tmA, tmB, tmBlo, tmAlo, em, p, majors, grid, smem, stream);
 }
 
 }  // namespace mdm

@@ -2,7 +2,8 @@
 
   python tools/gemm_bitwise.py dump OUT.npz [--root TREE]   run every non-atomic case of tests/gemm_cases.py,
                                                             tests/test_gemm_split_gpu.py and
-                                                            tests/test_gemm_epilogue_gpu.py with the library built in
+                                                            tests/test_gemm_epilogue_gpu.py and
+                                                            tests/test_gemm_epilogue_tma_gpu.py with the library built in
                                                             TREE (default: this repository) and store the outputs
   python tools/gemm_bitwise.py compare A.npz B.npz          exit 1 unless every stored output is bit-identical
 
@@ -39,6 +40,7 @@ def dump(out, root):
 
     import gemm_cases
     import test_gemm_epilogue_gpu
+    import test_gemm_epilogue_tma_gpu
     import test_gemm_split_gpu
 
     def split_k(fn):  # the case asks for nsplit > 1
@@ -48,6 +50,8 @@ def dump(out, root):
     cases = [(f"gemm_cases.{n}", gemm_cases, fn) for n, fn in gemm_cases.CASES if not split_k(fn)]
     cases += [(f"split_planes.{n}", test_gemm_split_gpu, fn) for n, fn in test_gemm_split_gpu.CASES]
     cases += [(f"epilogue.{n}", test_gemm_epilogue_gpu, fn) for n, fn in test_gemm_epilogue_gpu.CASES]
+    # run_plain / run_conv of test_gemm_epilogue_gpu make these cases' buffers
+    cases += [(f"epilogue_tma.{n}", test_gemm_epilogue_gpu, fn) for n, _, fn in test_gemm_epilogue_tma_gpu.CASES]
     arrays = {}
     for name, mod, fn in cases:
         rec = _RecordingTorch(torch)
