@@ -168,8 +168,8 @@ int mdm_net_weights_changed(mdm_net* net);
 typedef struct mdm_net_io {
   int32_t batch;
   int32_t tokens;
-  int32_t res[MDM_MAX_LEVELS];      /* image side per level, outermost (largest) first */
-  const float* x_t[MDM_MAX_LEVELS]; /* NCHW fp32, (batch, in_channels, res, res) */
+  int32_t res[MDM_MAX_LEVELS];      /* image height per level, outermost (largest) first; width: res_w */
+  const float* x_t[MDM_MAX_LEVELS]; /* NCHW fp32, (batch, in_channels, res, res_w) */
   const int64_t* times;             /* (batch,) */
   const float* lm;                  /* (batch, tokens, lm_dim) fp32 */
   const float* lm_mask;             /* (batch, tokens) fp32 0/1, or NULL */
@@ -185,6 +185,12 @@ typedef struct mdm_net_io {
   /* 1: lm is the raw encoder output and is multiplied by lm_mask on the way in (what language_models/factory.py:101
    * does as a separate (B,S,D) pass before the model is called); needs lm_mask and the lm_proj layer. */
   int32_t apply_lm_mask;
+  /* Image width per level (0 => res[l], a square image). Both sides must divide by the level's downsampling
+   * 2^(num_res - 1), and the bottleneck of an outer level must equal the next level's (res, res_w). */
+  int32_t res_w[MDM_MAX_LEVELS];
+  /* DiffusionConfig.model_output_scale (diffusion.py:83-85): s != 0 returns s * tanh(out / s) at every level, and
+   * the backward multiplies the incoming output gradient by 1 - (out / s)^2. 0 = off. */
+  float output_scale;
   /* 1: apply each level's ResNet dropout (the module is in training mode; independent of save_for_backward).
    * Element i of the [level_batch][H][W][C] output of a ResNet's SiLU(norm2) is kept when Philox4x32-10 with
    * key = dropout_seed and counter = (i / 4, stream id) gives a word w (word i % 4) with w / 2^32 >= p; the stream id
@@ -195,8 +201,8 @@ typedef struct mdm_net_io {
 } mdm_net_io;
 
 /* CUDA-graph execution of forward / backward (off by default). With it on, the first call with a given shape
- * signature (batch, per-level batch, resolutions, tokens, mask presence, which micro keys have values,
- * save_for_backward, dropout, stage,
+ * signature (batch, per-level batch, per-level height and width, tokens, mask presence, which micro keys have
+ * values, save_for_backward, dropout, output_scale, stage,
  * cond_cache, cond_emb presence; stage-1 calls always run eagerly) runs
  * eagerly, the
  * second is captured and later ones replay the captured graphs: inputs / output gradients are copied into static

@@ -1657,8 +1657,11 @@ __global__ void upsample2x_bwd_kernel(const float* __restrict__ dy, float* __res
   }
 }
 
+// TANH: model_output_scale s (diffusion.py:83-85): y = s * tanh(x / s) with the accurate tanhf, also written to keep
+// (the NCHW output the backward seed reads) when keep is not null
+template <bool TANH>
 __global__ void nhwc_to_nchw_kernel(const float* __restrict__ x, int ldc, float* __restrict__ y, int N, int C,
-                                    int HW) {
+                                    int HW, float s, float* __restrict__ keep) {
   const long long total = static_cast<long long>(N) * C * HW;
   long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   const long long gs = static_cast<long long>(gridDim.x) * blockDim.x;
@@ -1667,11 +1670,24 @@ __global__ void nhwc_to_nchw_kernel(const float* __restrict__ x, int ldc, float*
     const long long t = i / HW;
     const int c = static_cast<int>(t % C);
     const int n = static_cast<int>(t / C);
-    y[i] = x[(static_cast<long long>(n) * HW + p) * ldc + c];
+    float v = x[(static_cast<long long>(n) * HW + p) * ldc + c];
+    if (TANH) {
+      v = s * tanhf(v / s);
+      if (keep != nullptr) keep[i] = v;
+    }
+    y[i] = v;
   }
 }
+// d out / d o of y = s * tanh(o / s), from y itself: 1 - (y / s)^2
+__device__ __forceinline__ float tanh_scale_grad(float y, float s) {
+  const float t = y / s;
+  return 1.f - t * t;
+}
+// TANH: the incoming gradient is multiplied by tanh_scale_grad(yk, s), yk in the layout of x, before the scale
+template <bool TANH>
 __global__ void nchw_to_nhwc_f16_kernel(const float* __restrict__ x, const float* __restrict__ scale,
-                                        __half* __restrict__ y, int ldo, int N, int C, int HW) {
+                                        __half* __restrict__ y, int ldo, int N, int C, int HW, float s,
+                                        const float* __restrict__ yk) {
   const long long total = static_cast<long long>(N) * HW * ldo;
   long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   const long long gs = static_cast<long long>(gridDim.x) * blockDim.x;
@@ -1681,7 +1697,14 @@ __global__ void nchw_to_nhwc_f16_kernel(const float* __restrict__ x, const float
     const long long t = i / ldo;
     const int p = static_cast<int>(t % HW);
     const int n = static_cast<int>(t / HW);
-    y[i] = c < C ? __float2half_rn(sc * x[(static_cast<long long>(n) * C + c) * HW + p]) : __float2half_rn(0.f);
+    if (c >= C) {
+      y[i] = __float2half_rn(0.f);
+      continue;
+    }
+    const long long src = (static_cast<long long>(n) * C + c) * HW + p;
+    float g = x[src];
+    if (TANH) g *= tanh_scale_grad(yk[src], s);
+    y[i] = __float2half_rn(sc * g);
   }
 }
 
@@ -1792,13 +1815,14 @@ __global__ void unpack_conv_in_wgrad_kernel(const float* __restrict__ packed, fl
 }
 
 // ------------------------------------------------------------------ gradient scale
+template <bool TANH>
 __global__ void __launch_bounds__(256) grad_amax_kernel(const float* __restrict__ g, long long n,
-                                                        float* __restrict__ amax) {
+                                                        float* __restrict__ amax, float s, const float* __restrict__ yk) {
   float m = 0.f;
   long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   const long long gs = static_cast<long long>(gridDim.x) * blockDim.x;
   for (; i < n; i += gs) {
-    const float v = fabsf(g[i]);
+    const float v = TANH ? fabsf(g[i] * tanh_scale_grad(yk[i], s)) : fabsf(g[i]);
     if (v < INFINITY) m = fmaxf(m, v);  // skips NaN/Inf
   }
   m = warp_max(m);
@@ -2162,14 +2186,22 @@ void upsample2x_bwd(const float* dy, float* dx, int acc, int N, int H, int W, in
   upsample2x_bwd_kernel<<<grid_for(static_cast<long long>(N) * H * W * (C / 4)), 256, 0, st>>>(dy, dx, acc, N, H, W, C);
   MDM_LAUNCHED();
 }
-void nhwc_to_nchw(const float* x, int ldc, float* y, int N, int C, int HW, cudaStream_t st) {
-  nhwc_to_nchw_kernel<<<grid_for(static_cast<long long>(N) * C * HW), 256, 0, st>>>(x, ldc, y, N, C, HW);
+void nhwc_to_nchw(const float* x, int ldc, float* y, int N, int C, int HW, cudaStream_t st, float tanh_scale,
+                  float* keep) {
+  const unsigned grid = grid_for(static_cast<long long>(N) * C * HW);
+  if (tanh_scale != 0.f)
+    nhwc_to_nchw_kernel<true><<<grid, 256, 0, st>>>(x, ldc, y, N, C, HW, tanh_scale, keep);
+  else
+    nhwc_to_nchw_kernel<false><<<grid, 256, 0, st>>>(x, ldc, y, N, C, HW, 0.f, nullptr);
   MDM_LAUNCHED();
 }
 void nchw_to_nhwc_f16(const float* x_nchw, const float* scale, __half* y16, int ldo, int N, int C, int HW,
-                      cudaStream_t st) {
-  nchw_to_nhwc_f16_kernel<<<grid_for(static_cast<long long>(N) * HW * ldo), 256, 0, st>>>(x_nchw, scale, y16, ldo, N,
-                                                                                         C, HW);
+                      cudaStream_t st, float tanh_scale, const float* y_out) {
+  const unsigned grid = grid_for(static_cast<long long>(N) * HW * ldo);
+  if (tanh_scale != 0.f && y_out != nullptr)
+    nchw_to_nhwc_f16_kernel<true><<<grid, 256, 0, st>>>(x_nchw, scale, y16, ldo, N, C, HW, tanh_scale, y_out);
+  else
+    nchw_to_nhwc_f16_kernel<false><<<grid, 256, 0, st>>>(x_nchw, scale, y16, ldo, N, C, HW, 0.f, nullptr);
   MDM_LAUNCHED();
 }
 void sample_inv_std(const float* x, float* inv_std, int N, long long per, cudaStream_t st) {
@@ -2209,8 +2241,12 @@ void unpack_conv_in_wgrad(const float* packed, float* g_oihw, int Co, int Ci, co
   MDM_LAUNCHED();
 }
 
-void grad_amax(const float* g, long long n, float* amax_buf, cudaStream_t st) {
-  grad_amax_kernel<<<grid_for(n, 256, 132 * 4), 256, 0, st>>>(g, n, amax_buf);
+void grad_amax(const float* g, long long n, float* amax_buf, cudaStream_t st, float tanh_scale, const float* y_out) {
+  const unsigned grid = grid_for(n, 256, 132 * 4);
+  if (tanh_scale != 0.f && y_out != nullptr)
+    grad_amax_kernel<true><<<grid, 256, 0, st>>>(g, n, amax_buf, tanh_scale, y_out);
+  else
+    grad_amax_kernel<false><<<grid, 256, 0, st>>>(g, n, amax_buf, 0.f, nullptr);
   MDM_LAUNCHED();
 }
 void grad_scale_finalize(const float* amax_buf, float* scale, float* inv_scale, cudaStream_t st) {

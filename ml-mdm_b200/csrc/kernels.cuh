@@ -146,10 +146,13 @@ void im2col_input(const float* x_nchw, const float* inv_std, __half* col16, int 
 void upsample2x_f16(const float* x, __half* y16, int N, int H, int W, int C, cudaStream_t st);
 // dx[n,h,w,c] (+)= sum of the 2x2 block of dy (backward of nearest x2)
 void upsample2x_bwd(const float* dy, float* dx, int acc, int N, int H, int W, int C, cudaStream_t st);
-void nhwc_to_nchw(const float* x, int ldc, float* y, int N, int C, int HW, cudaStream_t st);
-// dy16[pix][ldo] = half(scale * dy_nchw) (columns >= C zero-filled)
+// tanh_scale = s != 0 (model_output_scale): y = s * tanh(x / s), also stored to keep when keep != nullptr
+void nhwc_to_nchw(const float* x, int ldc, float* y, int N, int C, int HW, cudaStream_t st, float tanh_scale = 0.f,
+                  float* keep = nullptr);
+// dy16[pix][ldo] = half(scale * dy_nchw) (columns >= C zero-filled); with tanh_scale = s != 0 and y_out (the NCHW
+// output s * tanh(o / s)) dy_nchw is first multiplied by 1 - (y_out / s)^2
 void nchw_to_nhwc_f16(const float* x_nchw, const float* scale, __half* y16, int ldo, int N, int C, int HW,
-                      cudaStream_t st);
+                      cudaStream_t st, float tanh_scale = 0.f, const float* y_out = nullptr);
 // per-sample unbiased std over (C,H,W): inv_std[n] = 1/std  (nested_unet.py:872)
 void sample_inv_std(const float* x, float* inv_std, int N, long long per, cudaStream_t st);
 
@@ -169,7 +172,9 @@ void unpack_conv_in_wgrad(const float* packed, float* g_oihw, int Co, int Ci, co
 
 // ---- gradient scaling: scale = 2^k with amax(|g|) * scale in [2^3, 2^4); inv = 1/scale.
 // amax_buf must be zero on entry; call grad_amax for every tensor, then grad_scale_finalize.
-void grad_amax(const float* g, long long n, float* amax_buf, cudaStream_t st);
+// tanh_scale / y_out as in nchw_to_nhwc_f16: the max is taken over g * (1 - (y_out / s)^2)
+void grad_amax(const float* g, long long n, float* amax_buf, cudaStream_t st, float tanh_scale = 0.f,
+               const float* y_out = nullptr);
 void grad_scale_finalize(const float* amax_buf, float* scale, float* inv_scale, cudaStream_t st);
 
 }  // namespace mdm

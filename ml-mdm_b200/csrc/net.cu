@@ -135,14 +135,17 @@ struct Net {
   struct OutRec {
     float* nhwc = nullptr;  // [pix][out_ch]
     __half* d16 = nullptr;  // [pix][8] scaled gradient (filled by backward)
-    int res = 0;
+    int h = 0, w = 0;
     int batch = 0;
+    float scale = 0.f;      // model_output_scale of the forward; != 0: y holds its NCHW output s * tanh(o / s)
+    float* y = nullptr;
   } outs[MDM_MAX_LEVELS];
   // samples level li processes (mixed-resolution batches run only a leading part of the batch on outer levels)
   int level_batch(int li) const {
     const int b = io->level_batch[li];
     return b > 0 ? b : io->batch;
   }
+  static int width_of(const mdm_net_io* q, int l) { return q->res_w[l] > 0 ? q->res_w[l] : q->res[l]; }
 
   ~Net() {
     for (cudaEvent_t e : eng.events) cudaEventDestroy(e);
@@ -1644,20 +1647,20 @@ struct Net {
   Act* level_fwd(int li, Act* x_feat) {
     Engine& E = eng;
     const LevelSpec& L = levels[li];
-    const int B = level_batch(li), R = io->res[li], C0 = L.c.channels[0];
+    const int B = level_batch(li), H = io->res[li], W = width_of(io, li), C0 = L.c.channels[0];
     MDM_CHECK(x_feat == nullptr || x_feat->n == B, "x_feat batch");
     LevelStep* ls = temb_fwd(L, B);
     // conv_in (+ x_feat when nested)  (unet.py:867-874,946-950; nested_unet.py:184-188)
     float* inv_std = nullptr;
     if (li < cfg.num_levels - 1 && !L.c.skip_normalization) {
       inv_std = E.alloc<float>(B);
-      sample_inv_std(io->x_t[li], inv_std, B, static_cast<long long>(cfg.in_channels) * R * R, E.st);
+      sample_inv_std(io->x_t[li], inv_std, B, static_cast<long long>(cfg.in_channels) * H * W, E.st);
     }
-    const long long rows = static_cast<long long>(B) * R * R;
+    const long long rows = static_cast<long long>(B) * H * W;
     __half* col = E.alloc<__half>(rows * 32);
-    im2col_input(io->x_t[li], inv_std, col, B, cfg.in_channels, R, R, E.st);
+    im2col_input(io->x_t[li], inv_std, col, B, cfg.in_channels, H, W, E.st);
     Param &ciw = P(L.pre + "conv_in.weight"), &cib = P(L.pre + "conv_in.bias");
-    Act* x = E.new_act(B, R, R, C0);
+    Act* x = E.new_act(B, H, W, C0);
     {
       Epi e;
       e.bias = cib.w;
@@ -1707,14 +1710,15 @@ struct Net {
       for (auto& b : L.mid) x = block_fwd(L, ls, b, x, nullptr, nullptr);
     } else {
       MDM_CHECK(L.mid.empty(), "outer levels of a nest have no mid blocks");
-      const int N = x->n, H = x->h, W = x->w, Co = x->c;
+      const int N = x->n, Hb = x->h, Wb = x->w, Co = x->c;
       const int Ci = levels[li + 1].c.channels[0];
-      MDM_CHECK(H == io->res[li + 1], "outer bottleneck resolution must equal the inner image size");
+      MDM_CHECK(Hb == io->res[li + 1] && Wb == width_of(io, li + 1),
+                "outer bottleneck resolution must equal the inner image size (both sides)");
       __half* x16 = E.alloc<__half>(x->numel());
       cast_f32_to_f16(x->p, x16, x->numel(), E.st);
       const int Bin = level_batch(li + 1);  // >= N; the inner level's extra samples see a zero feature
       MDM_CHECK(Bin >= N, "level_batch must not decrease from outer to inner levels");
-      Act* xin = conv_act(L.pre + "in_adapter.weight", L.pre + "in_adapter.bias", x16, N, H, W, Co, Ci, nullptr, Bin);
+      Act* xin = conv_act(L.pre + "in_adapter.weight", L.pre + "in_adapter.bias", x16, N, Hb, Wb, Co, Ci, nullptr, Bin);
       Act* xo_in = x;
       if (E.training) {
         const LevelSpec* Lp = &L;
@@ -1734,10 +1738,10 @@ struct Net {
       Act* feat = level_fwd(li + 1, xin);
       // out_adapter on the leading N samples only: the reference convolves all Bin and slices [:N] (nested_unet.py:208-209),
       // so the dropped rows contribute neither to the output nor to any gradient
-      const long long lead = static_cast<long long>(N) * H * W * Ci;
+      const long long lead = static_cast<long long>(N) * Hb * Wb * Ci;
       __half* f16 = E.alloc<__half>(lead);
       cast_f32_to_f16(feat->p, f16, lead, E.st);
-      Act* xn = conv_act(L.pre + "out_adapter.weight", L.pre + "out_adapter.bias", f16, N, H, W, Ci, Co, x->p);
+      Act* xn = conv_act(L.pre + "out_adapter.weight", L.pre + "out_adapter.bias", f16, N, Hb, Wb, Ci, Co, x->p);
       if (E.training) {
         const LevelSpec* Lp = &L;
         E.tape.push_back([=]() {
@@ -1770,7 +1774,7 @@ struct Net {
     // head (unet.py:876-880)
     Act* feat = x;
     {
-      const int Cf = feat->c, HW = R * R;
+      const int Cf = feat->c, HW = H * W;
       Param &nw = P(L.pre + "norm_out.weight"), &nb = P(L.pre + "norm_out.bias");
       Param &ow = P(L.pre + "conv_out.weight"), &ob = P(L.pre + "conv_out.bias");
       GnOut g = gn_fwd(Src2{feat->p, nullptr, Cf, 0}, B, HW, L.c.groups, nw, nb, nullptr, 0, 0, 1, false);
@@ -1779,11 +1783,17 @@ struct Net {
       Epi e;
       e.bias = ob.w;
       e.out_f32 = o;
-      E.conv3x3_fwd(g.y16, Cf, B, R, R, Cf, ow.w16, oc, e, ow.w16f, ow.bias_f);
-      nhwc_to_nchw(o, oc, io->out[li], B, oc, HW, E.st);
+      E.conv3x3_fwd(g.y16, Cf, B, H, W, Cf, ow.w16, oc, e, ow.w16f, ow.bias_f);
+      // model_output_scale: s * tanh(o / s) on the way out; a training forward keeps that output for the backward seed
+      const float s = io->output_scale;
+      float* keep = s != 0.f && E.training ? E.alloc<float>(rows * oc) : nullptr;
+      nhwc_to_nchw(o, oc, io->out[li], B, oc, HW, E.st, s, keep);
       E.rel(o);
-      outs[li].res = R;
+      outs[li].h = H;
+      outs[li].w = W;
       outs[li].batch = B;
+      outs[li].scale = s;
+      outs[li].y = keep;
       if (E.training) {
         const LevelSpec* Lp = &L;
         OutRec* orec = &outs[li];
@@ -1797,14 +1807,14 @@ struct Net {
           if (ob.g != nullptr) axpy_f32(ob.g, bs, 1.f, oc, 1, E.st);
           if (ow.g != nullptr) {
             float* wtmp = E.alloc<float>(9ll * Cf * oc);
-            E.conv3x3_wgrad(orec->d16, 8, g.y16, Cf, B, R, R, Cf, oc, wtmp);
+            E.conv3x3_wgrad(orec->d16, 8, g.y16, Cf, B, H, W, Cf, oc, wtmp);
             unpack_conv_wgrad(wtmp, ow.g, oc, Cf, 9, Cf, inv_scale(), E.st);
             E.rel(wtmp);
           }
           float* da = E.alloc<float>(rows * Cf);
           Epi e;
           e.out_f32 = da;
-          E.conv3x3_dgrad(orec->d16, 8, B, R, R, oc, ow.w16, Cf, e);
+          E.conv3x3_dgrad(orec->d16, 8, B, H, W, oc, ow.w16, Cf, e);
           gn_bwd(Src2{feat->p, nullptr, Cf, 0}, da, false, B, HW, Lp->c.groups, g.sums, nw, nb, nullptr, 0, 0, 1, nullptr,
                  nullptr, feat, nullptr);
           E.rel(da);
@@ -1835,7 +1845,9 @@ struct Net {
     for (int l = 0; l < cfg.num_levels; ++l) {
       MDM_CHECK(level_batch(l) >= 1 && level_batch(l) <= io->batch, "level_batch out of range");
       MDM_CHECK(io->x_t[l] != nullptr && io->out[l] != nullptr, "missing x_t/out pointer");
-      MDM_CHECK(io->res[l] % (1 << (cfg.levels[l].num_res - 1)) == 0, "resolution not divisible by the level's downsampling");
+      const int f = 1 << (cfg.levels[l].num_res - 1);
+      MDM_CHECK(io->res[l] > 0 && io->res_w[l] >= 0 && io->res[l] % f == 0 && width_of(io, l) % f == 0,
+                "image height and width must both divide by the level's downsampling");
     }
     if (cfg.cond_dim > 0 && io->stage == 0) MDM_CHECK(io->lm != nullptr && io->tokens > 0, "conditioning required");
     if (cfg.cond_dim > 0 && io->stage == 2)
@@ -1861,16 +1873,21 @@ struct Net {
     MDM_CUDA(cudaMemsetAsync(eng.d_amax, 0, sizeof(float), st));
     for (int l = 0; l < cfg.num_levels; ++l) {
       if (gio->dout[l] == nullptr) continue;
-      const long long n = static_cast<long long>(outs[l].batch) * cfg.out_channels * outs[l].res * outs[l].res;
-      grad_amax(gio->dout[l], n, eng.d_amax, st);
+      const long long n = static_cast<long long>(outs[l].batch) * cfg.out_channels * outs[l].h * outs[l].w;
+      // with model_output_scale the seed is dout * (1 - (y / s)^2): the power-of-two scale is chosen from that product
+      grad_amax(gio->dout[l], n, eng.d_amax, st, outs[l].scale, outs[l].y);
     }
     grad_scale_finalize(eng.d_amax, eng.d_scale, eng.d_inv_scale, st);
     for (int l = 0; l < cfg.num_levels; ++l) {
       if (gio->dout[l] == nullptr) continue;
-      const int HW = outs[l].res * outs[l].res;
+      const int HW = outs[l].h * outs[l].w;
       const int B = outs[l].batch;
       outs[l].d16 = eng.alloc<__half>(static_cast<long long>(B) * HW * 8);
-      nchw_to_nhwc_f16(gio->dout[l], eng.d_scale, outs[l].d16, 8, B, cfg.out_channels, HW, st);
+      nchw_to_nhwc_f16(gio->dout[l], eng.d_scale, outs[l].d16, 8, B, cfg.out_channels, HW, st, outs[l].scale, outs[l].y);
+      if (outs[l].y != nullptr) {
+        eng.rel(outs[l].y);
+        outs[l].y = nullptr;
+      }
     }
     replay_tape(tape_stage == 0);
     if (tape_stage == 2) {  // gradients of the caller's cond / cond_emb, unscaled
@@ -2012,7 +2029,8 @@ struct Net {
     int micro_mask = 0;  // bit k: the micro table's key k has values (staged in micro[k])
     int stage = 0, cond_cache = 0, has_cemb = 0;  // stage 2: the K/V cache mode and whether cond_emb is given
     uint64_t kv_epoch = 0;
-    int lb[MDM_MAX_LEVELS] = {0, 0, 0, 0}, res[MDM_MAX_LEVELS] = {0, 0, 0, 0};
+    int lb[MDM_MAX_LEVELS] = {0, 0, 0, 0}, res[MDM_MAX_LEVELS] = {0, 0, 0, 0}, res_w[MDM_MAX_LEVELS] = {0, 0, 0, 0};
+    float output_scale = 0.f;  // baked into the head kernels' arguments
     uint64_t bind_epoch = 0, pool_epoch = 0;
     float* x_t[MDM_MAX_LEVELS] = {nullptr, nullptr, nullptr, nullptr};
     float* out[MDM_MAX_LEVELS] = {nullptr, nullptr, nullptr, nullptr};
@@ -2076,10 +2094,14 @@ struct Net {
     if (r.training != (q->save_for_backward != 0) || r.batch != q->batch || r.tokens != q->tokens ||
         r.apply_lm_mask != (q->apply_lm_mask != 0) || r.dropout != (q->dropout != 0) ||
         r.has_mask != (key_mask(q) != nullptr) || r.micro_mask != micro_mask(q) || r.stage != q->stage ||
-        r.cond_cache != q->cond_cache || r.has_cemb != (q->stage == 2 && q->cond_emb != nullptr))
+        r.cond_cache != q->cond_cache || r.has_cemb != (q->stage == 2 && q->cond_emb != nullptr) ||
+        r.output_scale != q->output_scale)
       return false;
+    // both sides: a 32x48 and a 48x32 input move the same number of bytes but run different kernels
     for (int l = 0; l < cfg.num_levels; ++l)
-      if (r.res[l] != q->res[l] || r.lb[l] != (q->level_batch[l] > 0 ? q->level_batch[l] : q->batch)) return false;
+      if (r.res[l] != q->res[l] || r.res_w[l] != width_of(q, l) ||
+          r.lb[l] != (q->level_batch[l] > 0 ? q->level_batch[l] : q->batch))
+        return false;
     return true;
   }
   int find_rec(const StepIO* q) {
@@ -2103,10 +2125,12 @@ struct Net {
     r.has_cemb = q->stage == 2 && q->cond_emb != nullptr;
     r.apply_lm_mask = q->apply_lm_mask != 0;
     r.dropout = q->dropout != 0;
+    r.output_scale = q->output_scale;
     for (int l = 0; l < cfg.num_levels; ++l) {
       r.res[l] = q->res[l];
+      r.res_w[l] = width_of(q, l);
       r.lb[l] = q->level_batch[l] > 0 ? q->level_batch[l] : q->batch;
-      r.x_bytes[l] = sizeof(float) * static_cast<size_t>(r.lb[l]) * cfg.in_channels * r.res[l] * r.res[l];
+      r.x_bytes[l] = sizeof(float) * static_cast<size_t>(r.lb[l]) * cfg.in_channels * r.res[l] * r.res_w[l];
       MDM_CUDA(cudaMalloc(&r.x_t[l], r.x_bytes[l]));
       MDM_CUDA(cudaMalloc(&r.out[l], r.x_bytes[l] / cfg.in_channels * cfg.out_channels));
       if (r.training) MDM_CUDA(cudaMalloc(&r.dout[l], r.x_bytes[l] / cfg.in_channels * cfg.out_channels));

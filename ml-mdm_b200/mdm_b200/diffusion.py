@@ -98,8 +98,6 @@ class Model(nn.Module):
         super().__init__()
         self.diffusion_config = diffusion_config if diffusion_config is not None else DiffusionConfig()
         self._output_scale = self.diffusion_config.model_output_scale
-        if self._output_scale != 0:
-            raise NotImplementedError("model_output_scale (tanh output scaling) is 0 in every shipped config")
         self.vision_model = vision_model
         self.sampler = None
 
@@ -116,14 +114,25 @@ class Model(nn.Module):
     def input_channels(self):
         return self.vision_model.input_channels
 
+    def scaled_call(self, fn, *args):
+        """fn(*args) (the vision model or one of its methods) with the engine applying
+        s * tanh(out / s), s = model_output_scale, to the outputs and its derivative in the backward (diffusion.py:83-85)."""
+        vm = self.vision_model
+        vm.output_scale = float(self._output_scale or 0.0)
+        try:
+            return fn(*args)
+        finally:
+            vm.output_scale = 0.0
+
     def forward(self, x_t, times, lm_outputs, lm_mask, micros={}):
-        outputs = self.vision_model(x_t, times, lm_outputs, lm_mask, micros)
+        outputs = self.scaled_call(self.vision_model, x_t, times, lm_outputs, lm_mask, micros)
         # the reference allocates ones_like(outputs) here; a broadcast view keeps the interface
         return outputs, outputs.new_ones(()).expand_as(outputs)
 
 
 class NestedModel(Model):
-    """diffusion.py:251-292 with no_use_residual=True (the only working mode of the reference)."""
+    """diffusion.py:251-292 with no_use_residual=True (the only working mode of the reference). Its forward replaces
+    Model.forward, so model_output_scale is accepted and not applied, as in the reference."""
 
     def forward(self, x_t: List[torch.Tensor], times, lm_outputs, lm_mask, micros={}, mixed_ratio=None):
         if not self.diffusion_config.no_use_residual:

@@ -61,6 +61,8 @@ class NetIO(C.Structure):
         ("save_for_backward", C.c_int32),
         ("level_batch", C.c_int32 * MAX_LEVELS),
         ("apply_lm_mask", C.c_int32),
+        ("res_w", C.c_int32 * MAX_LEVELS),
+        ("output_scale", C.c_float),
         ("dropout", C.c_int32),
         ("dropout_seed", C.c_uint64),
     ]
@@ -198,7 +200,8 @@ class _DenoiseFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, native, nlev, need_grad, times, lm, mask, micro, *rest):
         xs = rest[:nlev]
-        outs = native._forward(list(xs), times, lm, mask, micro, save=need_grad, apply_lm_mask=native.apply_lm_mask)
+        outs = native._forward(list(xs), times, lm, mask, micro, save=need_grad, apply_lm_mask=native.apply_lm_mask,
+                               output_scale=native.output_scale)
         ctx.native = native
         ctx.nlev = nlev
         ctx.set_materialize_grads(False)
@@ -240,7 +243,7 @@ class _DenoisingFn(torch.autograd.Function):
     def forward(ctx, native, nlev, need_grad, cache, times, cond, cond_emb, cross_mask, micro, *rest):
         xs = rest[:nlev]
         outs = native._forward(list(xs), times, None, None, micro, save=need_grad, stage=2, cond=cond,
-                               cond_emb=cond_emb, cross_mask=cross_mask, cache=cache)
+                               cond_emb=cond_emb, cross_mask=cross_mask, cache=cache, output_scale=native.output_scale)
         ctx.native = native
         ctx.nlev = nlev
         ctx.want = (cond is not None and cond.requires_grad, cond_emb is not None and cond_emb.requires_grad)
@@ -306,6 +309,7 @@ class NativeNet:
         self._ready_cb = None
         self._keep = None
         self.apply_lm_mask = False
+        self.output_scale = 0.0  # model_output_scale of the forward being entered (diffusion.Model sets it)
         # ResNet dropout: the largest p of the nest, the modules whose train/eval flag it follows, and the
         # (flag, seed) of the forward being entered
         self.max_dropout = max(self.cfg.levels[i].dropout for i in range(self.cfg.num_levels))
@@ -405,9 +409,10 @@ class NativeNet:
             self.weights_epoch += 1
 
     # ---------------------------------------------------------------- public
-    def run(self, xs, times, lm, mask, micros, apply_lm_mask=False):
+    def run(self, xs, times, lm, mask, micros, apply_lm_mask=False, output_scale=0.0):
         self._bind()
         self.apply_lm_mask = bool(apply_lm_mask)
+        self.output_scale = float(output_scale)
         micro = self._enter(micros, xs[-1].shape[0])
         # (Function.forward runs with grad mode off, so the decision is taken here)
         need_grad = torch.is_grad_enabled() and any(p.requires_grad for p in self.params)
@@ -425,10 +430,11 @@ class NativeNet:
         cond, cemb = _ConditioningFn.apply(self, need_grad, bool(apply_lm_mask), lm, mask, *text)
         return cond, (cemb if self.cfg.has_cond_emb else None)
 
-    def run_denoising(self, xs, times, cond_emb, cond, cross_mask, micros):
+    def run_denoising(self, xs, times, cond_emb, cond, cross_mask, micros, output_scale=0.0):
         """forward_denoising on the engine (stage 2). Without autograd the K/V the cross-attention blocks compute from
         `cond` are kept by the engine and reused while `cond`, `cross_mask` and the weights stay what they were."""
         self._bind()
+        self.output_scale = float(output_scale)
         micro = self._enter(micros, xs[-1].shape[0])
         need_grad = torch.is_grad_enabled() and (any(p.requires_grad for p in self.params) or any(
             t is not None and t.requires_grad for t in (cond, cond_emb)))
@@ -493,7 +499,7 @@ class NativeNet:
         return micro
 
     def _forward(self, xs, times, lm, mask, micro, save, apply_lm_mask=False, stage=0, cond=None, cond_emb=None,
-                 cross_mask=None, cache=0):
+                 cross_mask=None, cache=0, output_scale=0.0):
         self._sync_weights()
         if save and self.graphs and self.grad_arena is not None:
             lo, hi = self.grad_arena.data_ptr(), self.grad_arena.data_ptr() + self.grad_arena.numel() * 4
@@ -515,14 +521,22 @@ class NativeNet:
         for i, x in enumerate(xs):
             if not x.is_cuda:
                 raise _lib.MdmError("inputs must be CUDA tensors")
+            if x.dim() != 4:
+                raise _lib.MdmError(f"level {i} input must be (batch, channels, height, width); got {tuple(x.shape)}")
+            if i > 0:
+                # the outer level's bottleneck feeds this level: both sides are the outer sides / 2^(num_res - 1)
+                r = 1 << (self.cfg.levels[i - 1].num_res - 1)
+                want = (xs[i - 1].shape[2] // r, xs[i - 1].shape[3] // r)
+                if tuple(x.shape[2:]) != want:
+                    raise _lib.MdmError(f"level {i} input is {tuple(x.shape[2:])} (height, width); the level above is "
+                                        f"{tuple(xs[i - 1].shape[2:])} and downsamples by {r}, so it must be {want}")
             x = f32(x)
-            if x.shape[2] != x.shape[3]:
-                raise _lib.MdmError("square images only")
             if not (1 <= x.shape[0] <= B) or (i > 0 and x.shape[0] < xs[i - 1].shape[0]):
                 raise _lib.MdmError("mixed-resolution batches: each level runs a leading part of the batch and inner "
                                     f"levels at least as many samples as outer ones; got {[t.shape[0] for t in xs]}")
             io.level_batch[i] = x.shape[0]
             io.res[i] = x.shape[2]
+            io.res_w[i] = x.shape[3]
             io.x_t[i] = x.data_ptr()
             o = torch.empty_like(x)
             outs.append(o)
@@ -560,6 +574,7 @@ class NativeNet:
             self._split_shapes = (tuple(cond.shape) if cond is not None else None, (B, td))
         io.apply_lm_mask = int(bool(apply_lm_mask))
         io.dropout, io.dropout_seed = self.dropout
+        io.output_scale = float(output_scale)
         st = torch.cuda.current_stream().cuda_stream
         _lib.check(self.lib.mdm_net_forward_micro(self.handle, C.byref(io), C.byref(sio) if stage else None,
                                                   C.byref(mio), C.c_void_p(st)), "mdm_net_forward_micro")

@@ -284,13 +284,14 @@ class UNet(nn.Module):
         return d
 
     def forward(self, x_t, times, conditioning=None, cond_mask=None, micros={}):
-        """UNet.forward (unet.py:971-987). x_t: (B, C, R, R) fp32 cuda tensor."""
+        """UNet.forward (unet.py:971-987). x_t: (B, C, H, W) fp32 cuda tensor; H and W divide by the downsampling."""
         single = not isinstance(x_t, (list, tuple))
         xs = [x_t] if single else list(x_t)
         # fuse_lm_mask: `conditioning` is the raw encoder output; the engine multiplies it by cond_mask on the way in
         # (language_models/factory.py:101 does that as a separate pass before the model is called)
         outs = self.native().run(xs, times, conditioning, cond_mask, micros,
-                                 apply_lm_mask=bool(getattr(self, "fuse_lm_mask", False)))
+                                 apply_lm_mask=bool(getattr(self, "fuse_lm_mask", False)),
+                                 output_scale=self._output_scale())
         return outs[0] if single else list(outs)
 
     def _require_top(self, what):
@@ -317,5 +318,11 @@ class UNet(nn.Module):
         self._require_top("forward_denoising")
         single = not isinstance(x_t, (list, tuple))
         xs = [x_t] if single else list(x_t)
-        outs = self.native().run_denoising(xs, times, cond_emb, conditioning, cond_mask, micros)
+        outs = self.native().run_denoising(xs, times, cond_emb, conditioning, cond_mask, micros,
+                                           output_scale=self._output_scale())
         return outs[0] if single else list(outs)
+
+    def _output_scale(self):
+        # model_output_scale, set by diffusion.Model around its own calls only: the reference applies s * tanh(out / s)
+        # in Model.forward (diffusion.py:83-85), so a U-Net called directly is never scaled
+        return float(getattr(self, "output_scale", 0.0))

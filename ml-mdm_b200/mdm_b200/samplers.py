@@ -264,9 +264,10 @@ class Sampler(nn.Module):
         from .diffusion import NestedModel
 
         cond_emb, cond, cmask = enc[2]
-        out = model.vision_model.forward_denoising(x_t, t, cond_emb, cond, cmask, micros)
-        if isinstance(model, NestedModel):
-            return out
+        vm = model.vision_model
+        if isinstance(model, NestedModel):  # NestedModel.forward applies no model_output_scale
+            return vm.forward_denoising(x_t, t, cond_emb, cond, cmask, micros)
+        out = model.scaled_call(vm.forward_denoising, x_t, t, cond_emb, cond, cmask, micros)
         return out, out.new_ones(()).expand_as(out)  # Model.forward's (outputs, variances placeholder)
 
     @staticmethod
@@ -422,7 +423,9 @@ class NestedSampler(Sampler):
             for i in range(1, len(x_t)):
                 outs.append(super()._postprocess(x_t[i], x0[i] if x0 is not None else None, extra,
                                                  yield_full=yield_full, clip=clip, image_scale=scales[i], **unused))
-            size = x_t[0].size(-1)
+            # both sides, for rectangles: a case the reference's nested pipeline never reaches (its gamma maps are
+            # resized to a square, samplers.py:618-622); for square images this is its int size
+            size = tuple(x_t[0].shape[-2:])
             if not yield_full:
                 out = torch.cat([F.interpolate(o, size, mode="bilinear") for o in outs[::-1]], -1)
             else:
