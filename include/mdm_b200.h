@@ -96,7 +96,8 @@ typedef struct mdm_gemm_params {
  * is bracketed by CUDA events on its stream; mdm_profile_read returns and clears their sum. */
 int mdm_profile_gemm(int enable);
 int mdm_profile_read(double* total_ms, long long* launches);
-/* Writes one CSV row per profiled launch (shape, grid parameters, milliseconds); call before mdm_profile_read. */
+/* Writes one CSV row per profiled launch (shape, grid parameters, milliseconds, and the lo planes it multiplied:
+ * planes = 0 none, 1 B lo, 2 A lo, 3 both); call before mdm_profile_read. */
 int mdm_profile_dump(const char* path);
 
 int mdm_gemm_raw(const mdm_tmap_spec* A, const mdm_tmap_spec* B, int a_mn, int b_mn,
@@ -191,6 +192,13 @@ typedef struct mdm_net_io {
   /* DiffusionConfig.model_output_scale (diffusion.py:83-85): s != 0 returns s * tanh(out / s) at every level, and
    * the backward multiplies the incoming output gradient by 1 - (out / s)^2. 0 = off. */
   float output_scale;
+  /* Operand precision of the weight products (what torch autocast asks of the reference's convs and linears, whose
+   * operands it rounds to bf16 / fp16). 0: weights enter every product as two fp16 planes, hi = fp16(w) and
+   * lo = fp16(w - hi), ~22 significant bits, and the ResNet data gradients that feed a GroupNorm backward as two planes
+   * too. 1: the hi planes only (11 bits; bf16 keeps 8): the weight products skip the B lo plane, the ResNet data
+   * gradients their A lo plane, and a weight refresh repacks the hi planes only (the lo planes are refilled before the
+   * next call with 0). The backward runs in the mode of its forward. */
+  int32_t single_plane;
   /* 1: apply each level's ResNet dropout (the module is in training mode; independent of save_for_backward).
    * Element i of the [level_batch][H][W][C] output of a ResNet's SiLU(norm2) is kept when Philox4x32-10 with
    * key = dropout_seed and counter = (i / 4, stream id) gives a word w (word i % 4) with w / 2^32 >= p; the stream id
@@ -202,7 +210,7 @@ typedef struct mdm_net_io {
 
 /* CUDA-graph execution of forward / backward (off by default). With it on, the first call with a given shape
  * signature (batch, per-level batch, per-level height and width, tokens, mask presence, which micro keys have
- * values, save_for_backward, dropout, output_scale, stage,
+ * values, save_for_backward, dropout, output_scale, single_plane, stage,
  * cond_cache, cond_emb presence; stage-1 calls always run eagerly) runs
  * eagerly, the
  * second is captured and later ones replay the captured graphs: inputs / output gradients are copied into static
@@ -242,7 +250,8 @@ typedef struct mdm_net_stage_io {
    * 1: the fp16 K/V every cross-attention block computes from cond are kept in net-owned memory (at fixed addresses,
    * so replayed graphs read them directly). 2: they are read from there; the token LayerNorm and every kv_cond
    * product are skipped and cond is not read. Mode 2 fails (nothing runs) unless a mode-1 call with the same batch,
-   * level_batch and tokens filled the slot and neither mdm_net_weights_changed nor mdm_net_bind_param came since.
+   * level_batch, tokens and mdm_net_io.single_plane filled the slot and neither mdm_net_weights_changed nor
+   * mdm_net_bind_param came since.
    * Whether cond itself is unchanged is the caller's to know. */
   int32_t cond_cache;
 } mdm_net_stage_io;

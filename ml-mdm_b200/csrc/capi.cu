@@ -34,15 +34,15 @@ int mdm_profile_gemm(int enable) {
 int mdm_profile_dump(const char* path) {
   FILE* f = fopen(path, "w");
   if (f == nullptr) return -1;
-  fprintf(f, "kind,majors,M,N,K,block_n,nz,nsplit,kblocks,H,W,nimg,ms\n");
+  fprintf(f, "kind,majors,M,N,K,block_n,nz,nsplit,kblocks,H,W,nimg,ms,planes\n");
   for (size_t i = 0; i < mdm::g_profile_events.size(); ++i) {
     auto& ev = mdm::g_profile_events[i];
     cudaEventSynchronize(ev.second);
     float ms = 0.f;
     cudaEventElapsedTime(&ms, ev.first, ev.second);
     const mdm_gemm_params& p = mdm::g_profile_params[i];
-    fprintf(f, "%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%.5f\n", p.kind, mdm::g_profile_majors[i], p.M, p.N, p.K, p.block_n,
-            p.nz1 * p.nz2, p.nsplit, p.num_kblocks, p.H, p.W, p.nimg, ms);
+    fprintf(f, "%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%.5f,%d\n", p.kind, mdm::g_profile_majors[i], p.M, p.N, p.K,
+            p.block_n, p.nz1 * p.nz2, p.nsplit, p.num_kblocks, p.H, p.W, p.nimg, ms, mdm::g_profile_planes[i]);
   }
   fclose(f);
   return 0;
@@ -53,6 +53,7 @@ int mdm_profile_read(double* total_ms, long long* launches) {
   long long n = 0;
   mdm::g_profile_params.clear();
   mdm::g_profile_majors.clear();
+  mdm::g_profile_planes.clear();
   for (auto& ev : mdm::g_profile_events) {
     cudaEventSynchronize(ev.second);
     float ms = 0.f;

@@ -195,7 +195,7 @@ void Engine::gemm_nt(const __half* A, long long lda, const __half* W, long long 
   fill_epi(p, e, N);
   TmapSpec a = spec(A, K, M, 1, 1, lda, lda * M, lda * M, 64, 128, 1, 1);
   TmapSpec b = spec(W, K, N, 1, 1, ldw, ldw * N, ldw * N, 64, p.block_n, 1, 1);
-  run(a, b, 0, 0, p, e, mt * ((N + p.block_n - 1) / p.block_n), st, lo_plane(W));
+  run(a, b, 0, 0, p, e, mt * ((N + p.block_n - 1) / p.block_n), st, b_lo(W));
 }
 
 void Engine::gemm_nn(const __half* A, long long lda, const __half* Bm, long long ldb, int M, int N, int K,
@@ -210,7 +210,7 @@ void Engine::gemm_nn(const __half* A, long long lda, const __half* Bm, long long
   fill_epi(p, e, N);
   TmapSpec a = spec(A, K, M, 1, 1, lda, lda * M, lda * M, 64, 128, 1, 1);
   TmapSpec b = spec(Bm, N, K, 1, 1, ldb, ldb * K, ldb * K, 64, 64, 1, 1);
-  run(a, b, 0, 1, p, e, mt * ((N + p.block_n - 1) / p.block_n), st, lo_plane(Bm));
+  run(a, b, 0, 1, p, e, mt * ((N + p.block_n - 1) / p.block_n), st, b_lo(Bm));
 }
 
 void Engine::gemm_tn(const __half* At, long long lda, const __half* Bm, long long ldb, int M, int N, int K,
@@ -265,7 +265,7 @@ void Engine::conv3x3_fwd(const __half* x16, int ldx, int N, int H, int W, int Ci
   TmapSpec a = spec(x16, Cin, W, H, N, ldx, static_cast<uint64_t>(W) * ldx, static_cast<uint64_t>(H) * W * ldx, 64,
                     p.PW, p.PH, 1);
   TmapSpec b = spec(w16, Cin, Cout, 9, 1, 9ull * Cin, Cin, 9ull * Cin * Cout, 64, p.block_n, 1, 1);
-  run(a, b, 0, 0, p, e, mt * ((Cout + p.block_n - 1) / p.block_n), st, lo_plane(w16));
+  run(a, b, 0, 0, p, e, mt * ((Cout + p.block_n - 1) / p.block_n), st, b_lo(w16));
 }
 
 void Engine::conv3x3_dgrad(const __half* dy16, int ldy, int N, int H, int W, int Cout, const __half* w16, int Cin,
@@ -292,7 +292,7 @@ void Engine::conv3x3_dgrad(const __half* dy16, int ldy, int N, int H, int W, int
   TmapSpec a = spec(dy16, Cout, W, H, N, ldy, static_cast<uint64_t>(W) * ldy, static_cast<uint64_t>(H) * W * ldy, 64,
                     p.PW, p.PH, 1);
   TmapSpec b = spec(w16, Cin, Cout, 9, 1, 9ull * Cin, Cin, 9ull * Cin * Cout, 64, 64, 1, 1);
-  run(a, b, 0, 1, p, e, mt * ((Cin + p.block_n - 1) / p.block_n), st, lo_plane(w16));
+  run(a, b, 0, 1, p, e, mt * ((Cin + p.block_n - 1) / p.block_n), st, b_lo(w16));
 }
 
 bool Engine::conv3x3_wgrad(const __half* dy16, int ldy, const __half* x16, int ldx, int N, int H, int W, int Cin,

@@ -119,6 +119,12 @@ struct Engine {
     if (a >= it->first + it->second * sizeof(__half)) return nullptr;
     return static_cast<const __half*>(p) + it->second;
   }
+  // Plane mode of the pass being recorded or replayed (mdm_net_io.single_plane): a single-plane pass multiplies the hi
+  // planes only, so its weight products get no B lo plane and its data gradients no A lo plane. A backward runs in the
+  // mode of the forward whose tape it replays.
+  bool single_plane = false;
+  // the B lo plane a weight product multiplies: lo_plane(p), or none in a single-plane pass
+  const __half* b_lo(const void* p) const { return single_plane ? nullptr : lo_plane(p); }
   bool training = false;
   std::vector<std::function<void()>> tape;
   std::deque<Act> acts;

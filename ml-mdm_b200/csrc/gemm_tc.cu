@@ -25,6 +25,7 @@ bool g_profile = false;
 std::vector<std::pair<cudaEvent_t, cudaEvent_t>> g_profile_events;
 std::vector<GemmParams> g_profile_params;  // parallel to g_profile_events
 std::vector<int> g_profile_majors;
+std::vector<int> g_profile_planes;
 
 using namespace ptx;
 
@@ -923,8 +924,8 @@ using GemmKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, 
 // majors (profile record): bit 1 = MN-major A, bit 0 = MN-major B, bit 2 = persistent kernel, bit 3 = staged epilogue,
 // bit 4 = TMA epilogue
 int launch_impl(GemmKernel k, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmBlo,
-                const CUtensorMap& tmAlo, const EpiMaps& em, const GemmParams& p, int majors, dim3 grid, size_t smem,
-                cudaStream_t stream) {
+                const CUtensorMap& tmAlo, const EpiMaps& em, const GemmParams& p, int majors, int planes, dim3 grid,
+                size_t smem, cudaStream_t stream) {
   static std::set<GemmKernel> attr_set;
   if (attr_set.count(k) == 0) {
     cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT);
@@ -943,6 +944,7 @@ int launch_impl(GemmKernel k, const CUtensorMap& tmA, const CUtensorMap& tmB, co
     g_profile_events.emplace_back(e0, e1);
     g_profile_params.push_back(p);
     g_profile_majors.push_back(majors);
+    g_profile_planes.push_back(planes);
   }
   ++g_launch_count;
   return static_cast<int>(cudaGetLastError());
@@ -1101,11 +1103,11 @@ int launch_gemm(const TmapSpec& A, const TmapSpec& Bin, int a_mn, int b_mn, cons
       return n;
     }();
     const long long ctas = std::min<long long>(tiles, std::max(1, num_sms - g_sm_reserve));
-    return launch_impl(k, tmA, tmB, tmBlo, tmAlo, em, p, majors, dim3(static_cast<unsigned>(ctas)), smem, stream);
+    return launch_impl(k, tmA, tmB, tmBlo, tmAlo, em, p, majors, planes, dim3(static_cast<unsigned>(ctas)), smem, stream);
   }
   dim3 grid(m_tiles, n_tiles, p.nz1 * p.nz2 * p.nsplit);
   if (grid.y > 65535 || grid.z > 65535) return -14;
-  return launch_impl(k, tmA, tmB, tmBlo, tmAlo, em, p, majors, grid, smem, stream);
+  return launch_impl(k, tmA, tmB, tmBlo, tmAlo, em, p, majors, planes, grid, smem, stream);
 }
 
 }  // namespace mdm

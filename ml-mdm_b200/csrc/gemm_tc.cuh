@@ -48,5 +48,6 @@ extern bool g_profile;
 extern std::vector<std::pair<cudaEvent_t, cudaEvent_t>> g_profile_events;
 extern std::vector<mdm_gemm_params> g_profile_params;
 extern std::vector<int> g_profile_majors;
+extern std::vector<int> g_profile_planes;  // PL_BLO | PL_ALO of each profiled launch
 
 }  // namespace mdm

@@ -82,6 +82,8 @@ struct Net {
   std::unordered_map<std::string, int> pindex;
   Engine eng;
   bool weights_dirty = true;
+  // the lo planes of the packed weights lag the fp32 masters: a single-plane pass repacked only the hi planes
+  bool lo_stale = false;
   bool fused_attention = getenv("MDM_UNFUSED_ATTENTION") == nullptr;
   bool have_tape = false;
   std::vector<void*> persistent;  // cudaMalloc'd for the life of the net
@@ -89,6 +91,7 @@ struct Net {
 
   // ---- split forward (mdm_net_stage_io.stage)
   int tape_stage = 0;          // stage (0 or 2) of the forward whose tape is held
+  bool tape_single = false;    // plane mode (mdm_net_io.single_plane) of that forward: its backward runs in it too
   Pool text_pool;              // workspace of the stage-1 passes, which run beside a held stage-0/2 tape
   bool have_cond_io = false;   // a stage-1 forward with save_for_backward ran: its backward recomputes from cond_io
   StepIO cond_io{};
@@ -101,6 +104,7 @@ struct Net {
   uint64_t kv_epoch = 0;       // bumped on reallocation: graphs that read or write the cache record it
   bool kv_valid = false;
   int kv_key[2 + MDM_MAX_LEVELS] = {0, 0, 0, 0, 0, 0};
+  bool kv_single = false;      // plane mode of the forward that filled it
 
   // per-step state
   struct CondStep {
@@ -447,8 +451,12 @@ struct Net {
   }
 
   // ---------------------------------------------------------------- weight packing
-  void prepare_weights() {
-    if (!weights_dirty) return;
+  // Packs the fp16 operand copies a pass in this plane mode reads. A single-plane pass packs the hi planes and leaves
+  // the lo planes stale (still allocated, so addresses baked into captured graphs stay valid); the next two-plane pass
+  // packs both again.
+  void prepare_weights(bool single) {
+    if (!weights_dirty && (single || !lo_stale)) return;
+    const bool lo = !single;
     cudaStream_t st = eng.st;
     for (auto& L : levels) {
       if (L.tl_w16 == nullptr && L.film_total > 0) {
@@ -467,18 +475,18 @@ struct Net {
       }
       if (p.pack == 1) {
         cast_f32_to_f16(p.w, p.w16, p.numel, st);
-        pack_lo(p.w, p.numel, p.w16, [&](const float* r, __half* lo) { cast_f32_to_f16(r, lo, p.numel, st); });
+        if (lo) pack_lo(p.w, p.numel, p.w16, [&](const float* r, __half* l) { cast_f32_to_f16(r, l, p.numel, st); });
       } else if (p.pack == 2) {
         const int Co = static_cast<int>(p.shape[0]), Ci = static_cast<int>(p.shape[1]);
         pack_conv_w(p.w, p.w16, Co, Ci, 9, st);
-        pack_lo(p.w, p.numel, p.w16, [&](const float* r, __half* lo) { pack_conv_w(r, lo, Co, Ci, 9, st); });
+        if (lo) pack_lo(p.w, p.numel, p.w16, [&](const float* r, __half* l) { pack_conv_w(r, l, Co, Ci, 9, st); });
         if (Engine::fold_ok(Ci, Co) && Co % 4 == 0) {  // narrow layer: W-folded copy + doubled bias (engine.cu)
           if (p.w16f == nullptr) {
             p.w16f = persist_w16(36ull * Co * Ci);
             p.bias_f = static_cast<float*>(persist(sizeof(float) * 2ull * Co));
           }
           pack_conv_w_fold(p.w, p.w16f, Co, Ci, st);
-          pack_lo(p.w, p.numel, p.w16f, [&](const float* r, __half* lo) { pack_conv_w_fold(r, lo, Co, Ci, st); });
+          if (lo) pack_lo(p.w, p.numel, p.w16f, [&](const float* r, __half* l) { pack_conv_w_fold(r, l, Co, Ci, st); });
           auto bi = pindex.find(p.name.substr(0, p.name.size() - 6) + "bias");  // "...weight" -> "...bias"
           MDM_CHECK(bi != pindex.end() && plist[bi->second].w != nullptr, "conv bias not bound");
           for (int r = 0; r < 2; ++r)
@@ -488,7 +496,7 @@ struct Net {
       else if (p.pack == 3) {
         const int Co = static_cast<int>(p.shape[0]), Ci = static_cast<int>(p.shape[1]);
         pack_conv_in_w(p.w, p.w16, Co, Ci, st);
-        pack_lo(p.w, p.numel, p.w16, [&](const float* r, __half* lo) { pack_conv_in_w(r, lo, Co, Ci, st); });
+        if (lo) pack_lo(p.w, p.numel, p.w16, [&](const float* r, __half* l) { pack_conv_in_w(r, l, Co, Ci, st); });
       }
     }
     for (auto& L : levels) {
@@ -499,7 +507,7 @@ struct Net {
           Param& bb = P(r.pre + ".time_layer.bias");
           w.w16 = L.tl_w16 + static_cast<size_t>(r.film_off) * td;
           cast_f32_to_f16(w.w, w.w16, w.numel, st);
-          pack_lo(w.w, w.numel, w.w16, [&](const float* r, __half* lo) { cast_f32_to_f16(r, lo, w.numel, st); });
+          if (lo) pack_lo(w.w, w.numel, w.w16, [&](const float* r, __half* l) { cast_f32_to_f16(r, l, w.numel, st); });
           MDM_CUDA(cudaMemcpyAsync(L.tl_bias + r.film_off, bb.w, sizeof(float) * 2 * r.cout,
                                    cudaMemcpyDeviceToDevice, st));
         }
@@ -517,7 +525,7 @@ struct Net {
           const int rows = 2 * a.C, D = cfg.cond_dim;
           if (kw.w16 == nullptr) kw.w16 = persist_w16(static_cast<size_t>(rows) * D);
           if (a.kv_bias_fold == nullptr) a.kv_bias_fold = static_cast<float*>(persist(sizeof(float) * rows));
-          fold_ln_weight(kw.w, lw.w, kw.w16, const_cast<__half*>(eng.lo_plane(kw.w16)), rows, D, st);
+          fold_ln_weight(kw.w, lw.w, kw.w16, lo ? const_cast<__half*>(eng.lo_plane(kw.w16)) : nullptr, rows, D, st);
           fold_ln_bias(kw.w, lb.w, kb.w, a.kv_bias_fold, rows, D, st);
         }
       };
@@ -526,6 +534,7 @@ struct Net {
       for (auto& b : L.up) fold_block(b);
     }
     weights_dirty = false;
+    lo_stale = single;
   }
 
   // ---------------------------------------------------------------- small building blocks
@@ -701,8 +710,9 @@ struct Net {
       // subtracts its group means, so an fp16 rounding here dominates the (cancelling) conv bias gradients before it
       float* da2 = E.alloc<float>(rows * cout);
       {
-        __half* d16lo = E.alloc<__half>(rows * cout);
-        f16_lo_plane(out->g, d16lo, rows * cout, E.st);
+        // (a single-plane pass takes the gradient at fp16 only)
+        __half* d16lo = E.single_plane ? nullptr : E.alloc<__half>(rows * cout);
+        if (d16lo != nullptr) f16_lo_plane(out->g, d16lo, rows * cout, E.st);
         Epi e;
         e.out_f32 = da2;
         e.a_lo = d16lo;
@@ -712,7 +722,7 @@ struct Net {
       // norm2 + FiLM + SiLU: h has a single consumer, so its gradient goes straight to the fp16 operand
       // of conv1's backward, with conv1's bias gradient as column sums
       __half* dh16 = E.alloc<__half>(rows * cout);
-      __half* dh16lo = E.alloc<__half>(rows * cout);
+      __half* dh16lo = E.single_plane ? nullptr : E.alloc<__half>(rows * cout);
       float* dfilm = E.alloc<float>(2ll * N * cout);
       gn_bwd(Src2{h, nullptr, cout, 0}, da2, false, N, HW, G, g2.sums, n2w, n2b, ls->film, Lp->film_total, r.film_off, 1,
              dfilm, nullptr, nullptr, nullptr, dh16, c1b.g, dh16lo, drop);
@@ -1858,7 +1868,9 @@ struct Net {
       eng.side_enabled = sw != nullptr ? atoi(sw) != 0 : true;
       eng.ev_next = 0;
     }
-    prepare_weights();
+    eng.single_plane = io->single_plane != 0;
+    tape_single = eng.single_plane;
+    prepare_weights(eng.single_plane);
     if (io->stage == 2) cond_input_fwd();
     else conditioning_fwd(0);
     level_fwd(0, nullptr);
@@ -1869,6 +1881,7 @@ struct Net {
   void backward_body(const mdm_net_grad_io* gio, cudaStream_t st) {
     MDM_CHECK(have_tape, "mdm_net_backward needs a preceding forward with save_for_backward=1");
     eng.st = st;
+    eng.single_plane = tape_single;
     // gradient scale from the largest |dout| (fp16 operands need the seed in range)
     MDM_CUDA(cudaMemsetAsync(eng.d_amax, 0, sizeof(float), st));
     for (int l = 0; l < cfg.num_levels; ++l) {
@@ -1915,10 +1928,12 @@ struct Net {
     std::vector<std::function<void()>> tape;
     CondStep cs;
     const StepIO* io;
-    bool training;
-    TextScope(Net* net, bool train) : n(net), cs(net->cs), io(net->io), training(net->eng.training) {
+    bool training, single;
+    TextScope(Net* net, bool train, bool single_plane)
+        : n(net), cs(net->cs), io(net->io), training(net->eng.training), single(net->eng.single_plane) {
       tape.swap(n->eng.tape);
       n->eng.training = train;
+      n->eng.single_plane = single_plane;
       n->text_pool.reset();
       n->eng.alt = &n->text_pool;
     }
@@ -1928,6 +1943,7 @@ struct Net {
       n->cs = cs;
       n->io = io;
       n->eng.training = training;
+      n->eng.single_plane = single;
     }
   };
 
@@ -1939,8 +1955,8 @@ struct Net {
     have_cond_io = false;
     eng.st = st;
     {
-      TextScope scope(this, false);
-      prepare_weights();
+      TextScope scope(this, false, q->single_plane != 0);
+      prepare_weights(q->single_plane != 0);
       io = q;
       conditioning_fwd(1);
       const long long n = static_cast<long long>(q->batch) * q->tokens * cfg.cond_dim;
@@ -1959,8 +1975,8 @@ struct Net {
     MDM_CHECK(have_cond_io, "a stage-1 backward needs a preceding stage-1 forward with save_for_backward=1");
     have_cond_io = false;
     eng.st = st;
-    TextScope scope(this, true);
-    prepare_weights();
+    TextScope scope(this, true, cond_io.single_plane != 0);  // the mode of the forward it differentiates
+    prepare_weights(cond_io.single_plane != 0);
     io = &cond_io;
     conditioning_fwd(1);
     Engine& E = eng;
@@ -1999,6 +2015,10 @@ struct Net {
         throw MdmFail("cond_cache 2: the K/V cache was filled for batch " + std::to_string(kv_key[0]) + ", tokens " +
                       std::to_string(kv_key[1]) + " (level batches " + std::to_string(kv_key[2]) + "..); this call has batch " +
                       std::to_string(q->batch) + ", tokens " + std::to_string(q->tokens));
+      if (kv_single != (q->single_plane != 0))
+        throw MdmFail(std::string("cond_cache 2: the K/V cache was filled by a ") + (kv_single ? "single" : "two") +
+                      "-plane forward; this call is " + (q->single_plane ? "single" : "two") +
+                      "-plane (mdm_net_io.single_plane): fill it again with cond_cache 1");
       return;
     }
     kv_valid = false;
@@ -2013,6 +2033,7 @@ struct Net {
       ++kv_epoch;
     }
     memcpy(kv_key, key, sizeof(key));
+    kv_single = q->single_plane != 0;
   }
   static int level_batch_of(const mdm_net_io* q, int l) { return q->level_batch[l] > 0 ? q->level_batch[l] : q->batch; }
 
@@ -2031,6 +2052,7 @@ struct Net {
     uint64_t kv_epoch = 0;
     int lb[MDM_MAX_LEVELS] = {0, 0, 0, 0}, res[MDM_MAX_LEVELS] = {0, 0, 0, 0}, res_w[MDM_MAX_LEVELS] = {0, 0, 0, 0};
     float output_scale = 0.f;  // baked into the head kernels' arguments
+    int single_plane = 0;      // which kernels and operand planes the weight products were captured with
     uint64_t bind_epoch = 0, pool_epoch = 0;
     float* x_t[MDM_MAX_LEVELS] = {nullptr, nullptr, nullptr, nullptr};
     float* out[MDM_MAX_LEVELS] = {nullptr, nullptr, nullptr, nullptr};
@@ -2095,7 +2117,7 @@ struct Net {
         r.apply_lm_mask != (q->apply_lm_mask != 0) || r.dropout != (q->dropout != 0) ||
         r.has_mask != (key_mask(q) != nullptr) || r.micro_mask != micro_mask(q) || r.stage != q->stage ||
         r.cond_cache != q->cond_cache || r.has_cemb != (q->stage == 2 && q->cond_emb != nullptr) ||
-        r.output_scale != q->output_scale)
+        r.output_scale != q->output_scale || r.single_plane != (q->single_plane != 0))
       return false;
     // both sides: a 32x48 and a 48x32 input move the same number of bytes but run different kernels
     for (int l = 0; l < cfg.num_levels; ++l)
@@ -2126,6 +2148,7 @@ struct Net {
     r.apply_lm_mask = q->apply_lm_mask != 0;
     r.dropout = q->dropout != 0;
     r.output_scale = q->output_scale;
+    r.single_plane = q->single_plane != 0;
     for (int l = 0; l < cfg.num_levels; ++l) {
       r.res[l] = q->res[l];
       r.res_w[l] = width_of(q, l);
@@ -2220,7 +2243,7 @@ struct Net {
       if (r.micro[k] != nullptr)
         MDM_CUDA(cudaMemcpyAsync(r.micro[k], io_->values[k], sizeof(float) * r.batch, cudaMemcpyDeviceToDevice, st));
     eng.st = st;
-    prepare_weights();  // outside the graph: only runs when the fp32 masters changed
+    prepare_weights(io_->single_plane != 0);  // outside the graph: only when the masters changed or lo planes are stale
     const bool valid = r.fwd != nullptr && r.bind_epoch == bind_epoch && r.pool_epoch == eng.pool.epoch() &&
                        (r.cond_cache == 0 || r.kv_epoch == kv_epoch) &&
                        (!r.training || (!r.bwd.empty() && r.bwd_notifies == (ready_fn != nullptr)));

@@ -63,6 +63,7 @@ class NetIO(C.Structure):
         ("apply_lm_mask", C.c_int32),
         ("res_w", C.c_int32 * MAX_LEVELS),
         ("output_scale", C.c_float),
+        ("single_plane", C.c_int32),
         ("dropout", C.c_int32),
         ("dropout_seed", C.c_uint64),
     ]
@@ -166,6 +167,14 @@ def build_net_cfg(module) -> NetCfg:
     return nc
 
 
+def autocast_active():
+    """Whether the call being entered runs inside an active CUDA autocast region (bf16 or fp16). The engine then runs
+    its weight products on the hi fp16 plane of the weights only (mdm_net_io.single_plane): autocast rounds the
+    reference's conv and linear operands to 8 (bf16) or 11 (fp16) significand bits, so the lo plane that carries the
+    weights to ~22 bits for the fp32 path buys nothing there."""
+    return torch.is_autocast_enabled("cuda")
+
+
 def _scale_only(mods):
     return all(m.conditions is None or list(m.conditions) == ["scale"] for m in mods)
 
@@ -195,13 +204,14 @@ def build_micro_cfg(module) -> MicroCfg:
 class _DenoiseFn(torch.autograd.Function):
     """One autograd node for the whole denoiser: forward = mdm_net_forward, backward = mdm_net_backward.
     Parameters are passed so autograd routes their gradients (DDP hooks, accumulation, clipping work
-    on ordinary .grad tensors)."""
+    on ordinary .grad tensors). The plane mode is read here, at forward time (autocast_active); the engine runs the
+    backward in the mode of its forward, so a backward called outside the autocast region still matches it."""
 
     @staticmethod
     def forward(ctx, native, nlev, need_grad, times, lm, mask, micro, *rest):
         xs = rest[:nlev]
         outs = native._forward(list(xs), times, lm, mask, micro, save=need_grad, apply_lm_mask=native.apply_lm_mask,
-                               output_scale=native.output_scale)
+                               output_scale=native.output_scale, single_plane=autocast_active())
         ctx.native = native
         ctx.nlev = nlev
         ctx.set_materialize_grads(False)
@@ -221,7 +231,9 @@ class _ConditioningFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, native, need_grad, apply_lm_mask, lm, mask, *text_params):
-        cond, cemb = native._conditioning(lm, mask, save=need_grad, apply_lm_mask=apply_lm_mask)
+        # (the engine recomputes the text path for the stage-1 backward in this mode)
+        cond, cemb = native._conditioning(lm, mask, save=need_grad, apply_lm_mask=apply_lm_mask,
+                                          single_plane=autocast_active())
         ctx.native = native
         ctx.set_materialize_grads(False)
         if not need_grad:
@@ -243,7 +255,8 @@ class _DenoisingFn(torch.autograd.Function):
     def forward(ctx, native, nlev, need_grad, cache, times, cond, cond_emb, cross_mask, micro, *rest):
         xs = rest[:nlev]
         outs = native._forward(list(xs), times, None, None, micro, save=need_grad, stage=2, cond=cond,
-                               cond_emb=cond_emb, cross_mask=cross_mask, cache=cache, output_scale=native.output_scale)
+                               cond_emb=cond_emb, cross_mask=cross_mask, cache=cache, output_scale=native.output_scale,
+                               single_plane=autocast_active())
         ctx.native = native
         ctx.nlev = nlev
         ctx.want = (cond is not None and cond.requires_grad, cond_emb is not None and cond_emb.requires_grad)
@@ -449,14 +462,15 @@ class NativeNet:
 
     def _kv_key(self, xs, cond, mask):
         # identity (a weak reference: a freed tensor's address is reused) and in-place version of the tokens and mask,
-        # the weight state, and the shapes the cache was laid out for
+        # the weight state, the shapes the cache was laid out for and the plane mode its K/V were computed in
         def ident(t):
             return None if t is None else (weakref.ref(t), t._version)
-        return (ident(cond), ident(mask), self.weights_epoch, tuple(x.shape[0] for x in xs), tuple(cond.shape))
+        return (ident(cond), ident(mask), self.weights_epoch, tuple(x.shape[0] for x in xs), tuple(cond.shape),
+                autocast_active())
 
     def _cache_mode(self, xs, cond, mask):
         """2 when the engine's K/V cache was filled from this very `cond` / `mask` (unchanged since) under the current
-        weights, else 1 (fill it)."""
+        weights and in the current plane mode, else 1 (fill it)."""
         self._sync_weights()  # an in-place weight update bumps weights_epoch here, before the comparison
         old = self._kv
         if old is None:
@@ -499,7 +513,7 @@ class NativeNet:
         return micro
 
     def _forward(self, xs, times, lm, mask, micro, save, apply_lm_mask=False, stage=0, cond=None, cond_emb=None,
-                 cross_mask=None, cache=0, output_scale=0.0):
+                 cross_mask=None, cache=0, output_scale=0.0, single_plane=False):
         self._sync_weights()
         if save and self.graphs and self.grad_arena is not None:
             lo, hi = self.grad_arena.data_ptr(), self.grad_arena.data_ptr() + self.grad_arena.numel() * 4
@@ -575,13 +589,14 @@ class NativeNet:
         io.apply_lm_mask = int(bool(apply_lm_mask))
         io.dropout, io.dropout_seed = self.dropout
         io.output_scale = float(output_scale)
+        io.single_plane = int(bool(single_plane))
         st = torch.cuda.current_stream().cuda_stream
         _lib.check(self.lib.mdm_net_forward_micro(self.handle, C.byref(io), C.byref(sio) if stage else None,
                                                   C.byref(mio), C.c_void_p(st)), "mdm_net_forward_micro")
         self._keep = keep if save else None  # inputs must outlive the tape
         return outs
 
-    def _conditioning(self, lm, mask, save, apply_lm_mask=False):
+    def _conditioning(self, lm, mask, save, apply_lm_mask=False, single_plane=False):
         """mdm_net_forward with stage 1: (cond, cond_emb); cond_emb is an empty tensor for a model without one."""
         self._sync_weights()
         io = NetIO()
@@ -605,6 +620,7 @@ class NativeNet:
             io.lm_mask = f32(mask).data_ptr()
         io.apply_lm_mask = int(bool(apply_lm_mask))
         io.save_for_backward = int(save)
+        io.single_plane = int(bool(single_plane))
         cond = torch.empty(B, S, self.cfg.cond_dim, device=lm.device, dtype=torch.float32)
         td = self.cfg.levels[self.cfg.num_levels - 1].temporal_dim
         cemb = torch.empty(B, td if self.cfg.has_cond_emb else 0, device=lm.device, dtype=torch.float32)

@@ -2,11 +2,13 @@
 the `args.fp16` branch the shipped cc12m_1024x1024.yaml selects), using the fused clip + Adam + EMA + zero-grad
 sweep when the optimizer is `mdm_b200.optim.FusedAdam` and the reference's separate calls otherwise.
 
-`args.fp16` in the reference means bf16 autocast + GradScaler around torch modules (trainer.py:29-61). The engine's
-arithmetic does not depend on autocast (fp16 operands, fp32 accumulation, its own power-of-two scaling of the
-backward seed), so that branch keeps the reference's *control flow* -- loss * loss_factor, the division by
-num_grad_accumulations before backward, a NaN loss that neither steps the optimizer nor the scheduler, clipping
-over model.model.parameters(), GradScaler scale/unscale/step/update when a scaler is passed -- on the same kernels."""
+`args.fp16` in the reference means "Using fp16 to speed-up training": get_loss under bf16 autocast, then GradScaler
+around the backward and the step (trainer.py:29-61). That branch does the same: the loss is computed inside
+torch.autocast("cuda", dtype=torch.bfloat16), which the native denoiser honours by running its weight products on the
+weights' hi fp16 plane only (models/native.py autocast_active; its backward follows the forward's mode), and it keeps
+the reference's control flow -- loss * loss_factor, the division by num_grad_accumulations before backward, a NaN loss
+that neither steps the optimizer nor the scheduler, clipping over model.model.parameters(), GradScaler
+scale/unscale/step/update when a scaler is passed."""
 import numpy as np
 import torch
 import torch.nn as nn
@@ -59,18 +61,19 @@ def train_batch(model, sample, optimizer, scheduler, logger, args, grad_scaler=N
 def _train_batch_fp16(model, sample, optimizer, scheduler, logger, args, grad_scaler, accumulate_gradient,
                       num_grad_accumulations, ema_model, loss_factor, lr):
     """trainer.py:29-61."""
-    losses, times, x_t, means, targets, weights = model.get_loss(sample)
-    if weights is None:
-        loss = losses.mean()
-    else:
-        loss = (losses * weights).sum() / weights.sum()
-    loss = loss * loss_factor
-    loss_val = loss.item()
-    if np.isnan(loss_val):  # trainer.py:39-41: no optimizer step, no scheduler step
-        optimizer.zero_grad()
-        return loss_val, losses, times, x_t, means, targets
-    if num_grad_accumulations != 1:
-        loss = loss / num_grad_accumulations
+    with torch.autocast("cuda", dtype=torch.bfloat16):
+        losses, times, x_t, means, targets, weights = model.get_loss(sample)
+        if weights is None:
+            loss = losses.mean()
+        else:
+            loss = (losses * weights).sum() / weights.sum()
+        loss = loss * loss_factor
+        loss_val = loss.item()
+        if np.isnan(loss_val):  # trainer.py:39-41: no optimizer step, no scheduler step
+            optimizer.zero_grad()
+            return loss_val, losses, times, x_t, means, targets
+        if num_grad_accumulations != 1:
+            loss = loss / num_grad_accumulations
     scaling = grad_scaler is not None and grad_scaler.is_enabled()
     (grad_scaler.scale(loss) if scaling else loss).backward()
     if not accumulate_gradient:
