@@ -115,9 +115,10 @@ def threshold_sample(sample, ratio=0.995, max_value=100.0):
     torch.quantile (third-party arithmetic, linear interpolation on fp32 ranks) is the anchor."""
     b = sample.shape[0]
     flat = sample.reshape(b, -1)
-    s = torch.quantile(flat.abs(), ratio, dim=1)
-    s = torch.clamp(s, min=1, max=max_value).unsqueeze(1)
-    return (torch.clamp(flat, -s, s) / s).reshape(sample.shape)
+    # tensor methods only, so that tests/algebra_cases.Mag (an fp64 value with its error magnitude) runs this too
+    s = flat.abs().quantile(ratio, dim=1)
+    s = s.clamp(min=1, max=max_value).unsqueeze(1)
+    return (flat.clamp(-s, s) / s).reshape(sample.shape)
 
 
 def clip_sample(x0, image_scale, mode):
@@ -173,16 +174,20 @@ def mixed_ratio_fractions(spec):
 
 
 def training_loss(net, P, images, eps_list, time, lm, mask, gammas, scales, ptype, ltype, shifted, power,
-                  weights=None, double_loss=True, mixed_ratio=None):
+                  weights=None, double_loss=True, mixed_ratio=None, rescale_signal=None):
     """Base (scales == [1]) or nested get_loss given the noise tensors. Returns (loss(B,), x_t list, outs).
-    mixed_ratio: cumulative fractions per level (diffusion.py:262-274, 378-382)."""
+    weights: per-level multi_res_weights (diffusion.py:368-374), double_loss: use_double_loss.
+    mixed_ratio: cumulative fractions per level (diffusion.py:262-274, 378-382).
+    rescale_signal (base pipeline only): x_t is made from images / r, the targets from the unrescaled images
+    (diffusion.py:156, 163-165)."""
     nested = len(scales) > 1
     ratios = [scales[0] // s for s in scales]
     imgs = nested_pyramid(images, ratios) if nested else [images]
     g_base = gammas[time + 1]
     gs = [shift_table(g_base, s, power) if (nested and shifted) else g_base for s in scales]
     divs = [1.0 if (not nested or shifted) else float(s) for s in scales]
-    x_t = [q_sample(x / d if d != 1.0 else x, e, g) for x, e, g, d in zip(imgs, eps_list, gs, divs)]
+    xdivs = [float(rescale_signal)] if (not nested and rescale_signal) else divs
+    x_t = [q_sample(x / d if d != 1.0 else x, e, g) for x, e, g, d in zip(imgs, eps_list, gs, xdivs)]
     B = images.shape[0]
     x_in = x_t
     if mixed_ratio is not None:  # NestedModel.forward: leading part of the batch per level, zero-padded predictions
@@ -207,12 +212,20 @@ def training_loss(net, P, images, eps_list, time, lm, mask, gammas, scales, ptyp
 
 
 def sample_loop(net, P, x_init, lm, mask, gammas, scales, ptype, n_diffusion, num_inference_steps, ddim_eta, clip=True,
-                shifted=False, power=1, guidance_scale=1.0):
-    """Deterministic (eta = 0) or seeded p_sample loop with resampled steps; x_init is a list per level."""
+                shifted=False, power=1, guidance_scale=1.0, rescale_signal=None, noises=None, tabs=None, trace=None):
+    """p_sample loop (samplers.py:516-578, 655-713) with resampled steps; x_init is a list per level. A full-length
+    loop is num_inference_steps == n_diffusion. Returns the final images per level, scaled and clipped as _postprocess
+    does (samplers.py:580-599, 715-739).
+    clip: the threshold mode (bool or ThresholdType name). noises: per step, the list of per-level noise tensors of
+    the stochastic steps (drawn from torch's generator when None). tabs: per-level gamma tables (default: gammas,
+    shifted per level when `shifted`). trace: a list that receives (x0 list, x_s list) of every step."""
     nested = len(scales) > 1
     ts = set_timesteps(n_diffusion, num_inference_steps)
     x_t = [x.clone() for x in x_init]
-    tabs = [shift_table(gammas, s, power) if (nested and shifted) else gammas for s in scales]
+    if tabs is None:
+        tabs = [shift_table(gammas, s, power) if (nested and shifted) else gammas for s in scales]
+    img_scales = [1.0 if shifted else float(sc) for sc in scales] if nested else \
+        [float(rescale_signal) if rescale_signal else 1.0]
     B = x_t[0].shape[0]
     with torch.no_grad():
         for i, t in enumerate(ts[:-1]):
@@ -226,11 +239,14 @@ def sample_loop(net, P, x_init, lm, mask, gammas, scales, ptype, n_diffusion, nu
             else:
                 o = net.forward(P, x_t if nested else x_t[0], times, lm, mask, {})
                 o = list(o) if nested else [o]
-            nxt = []
-            for x, p, tab, sc in zip(x_t, o, tabs, scales):
+            nxt, x0s = [], []
+            for lv, (x, p, tab, sc) in enumerate(zip(x_t, o, tabs, img_scales)):
                 need = (int(t) != 1) if nested else (int(s) != 0)
-                img_scale = 1.0 if (not nested or shifted) else float(sc)
-                _, xs = reverse_step(x, p, tab[int(t)], tab[int(s)], ptype, clip, img_scale, ddim_eta, need)
+                nz = noises[i][lv] if noises is not None else None
+                x0, xs = reverse_step(x, p, tab[int(t)], tab[int(s)], ptype, clip, sc, ddim_eta, need, noise=nz)
                 nxt.append(xs)
+                x0s.append(x0)
             x_t = nxt
-    return [x.clip(-1, 1) for x in x_t]
+            if trace is not None:
+                trace.append((x0s, nxt))
+    return [(x * sc).clip(-1, 1) if sc != 1.0 else x.clip(-1, 1) for x, sc in zip(x_t, img_scales)]
