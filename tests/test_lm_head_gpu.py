@@ -1,78 +1,39 @@
-"""lm_head (UNetConfig.num_lm_head_layers) on the GPU: the token self-attention operator against fp64 torch, and
-the native UNet / NestedUNet with lm_head layers against the oracle, the reference fixtures and graph replay."""
-import ctypes as C
-import math
+"""lm_head (UNetConfig.num_lm_head_layers) on the GPU: the token self-attention operator against the fp64
+restatement of SelfAttention1D.attention element by element (the bound of tests/attn_cases.py), and the native UNet /
+NestedUNet with lm_head layers against the oracle, the reference fixtures and graph replay."""
 import os
 import sys
 
 import pytest
 import torch
 
+import attn_cases as ac
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "..", "ml-mdm_b200"))
-from mdm_b200 import _lib  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
-TOL = 4e-3  # fp16 P / dS tiles and fp16 outputs, as for the spatial attention operator
 
-
-def ref_token_attention(qkv, mask, heads):
-    """SelfAttention1D.attention (reference models/unet.py:350-375): qkv (B,T,3D), mask (B,T) or None -> (B,T,D)."""
-    B, T, D3 = qkv.shape
-    D = D3 // 3
-    d = D // heads
-    q, k, v = (x.reshape(B, T, heads, d) for x in qkv.split(D, dim=2))
-    s = 1 / math.sqrt(math.sqrt(d))
-    w = torch.einsum("bthc,bshc->bhts", q * s, k * s)
-    if mask is not None:
-        w = w.masked_fill(mask.view(B, 1, 1, T) == 0, float("-inf"))
-    return torch.einsum("bhts,bshc->bthc", torch.softmax(w, -1), v).reshape(B, T, D)
-
-
-def run_op(B, T, d, masked, heads=8, seed=0):
-    D = d * heads
-    g = torch.Generator().manual_seed(seed)
-    qkv = (torch.randn(B, T, 3 * D, generator=g) * 0.7).half()
-    mask = None
-    if masked:
-        mask = torch.ones(B, T)
-        for i in range(B):
-            mask[i, max(1, T // 2 + i):] = 0  # every sample keeps at least one key
-    dO = (torch.randn(B, T, D, generator=g) * 0.5).half()
-    qr = qkv.double().requires_grad_(True)
-    out = ref_token_attention(qr, mask, heads)
-    (out * dO.double()).sum().backward()
-
-    dev = "cuda"
-    qc, dOc = qkv.to(dev), dO.to(dev)
-    mc = mask.to(dev) if mask is not None else None
-    o16 = torch.empty(B, T, D, device=dev, dtype=torch.float16)
-    stats = torch.empty(B, heads, T, 2, device=dev)
-    Dterm = torch.empty(B, heads, T, device=dev)
-    dq32 = torch.empty(B, T, D, device=dev)
-    dqkv = torch.empty(B, T, 3 * D, device=dev, dtype=torch.float16)
-    lib = _lib.lib()
-    st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-    P = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None
-    _lib.check(lib.mdm_op_token_attention_fwd(P(qc), P(mc), B, T, D, heads, P(o16), P(stats), st), "token attn fwd")
-    _lib.check(lib.mdm_op_token_attention_bwd(P(qc), P(mc), P(dOc), P(o16), P(stats), B, T, D, heads, P(Dterm),
-                                              P(dq32), P(dqkv), st), "token attn bwd")
-    torch.cuda.synchronize()
-
-    def rel(a, b):
-        return float((a.double().cpu() - b).abs().max() / b.abs().max().clamp_min(1e-30))
-
-    return {"out": rel(o16, out.detach()), "dqkv": rel(dqkv, qr.grad)}
+def check_token(name, spec):
+    ratios = ac.run_token(spec)
+    print(name, {k: round(v, 3) for k, v in ratios.items()})
+    for k, v in ratios.items():
+        assert v <= ac.C, (name, k, v)
 
 
 @pytest.mark.parametrize("masked", [False, True], ids=["unmasked", "masked"])
 @pytest.mark.parametrize("T", [1, 6, 77, 128, 200])
 @pytest.mark.parametrize("d", [8, 64, 128, 256])
 def test_token_attention_op(d, T, masked):
-    B = 4 if d * T <= 64 * 128 else 2
-    errs = run_op(B, T, d, masked, seed=d * 1000 + T)
-    assert all(v <= TOL for v in errs.values()), errs
+    check_token(f"d{d}_t{T}", ac.token_grid_spec(d, T, masked))
+
+
+@pytest.mark.parametrize("name", list(ac.TOKEN))
+def test_token_attention_case(name):
+    """Several key chunks with planted keys 127, 128 and T - 1, head widths 136 and 192 (a partly filled second
+    128-column half), and a sample whose keys are all masked (zero outputs and gradients)."""
+    check_token(name, ac.TOKEN[name])
 
 
 # ------------------------------------------------------------------------------------------ the network
