@@ -12,6 +12,7 @@
  *   mdm_set_timesteps    samplers.py:601-609
  *   mdm_q_sample*, mdm_loss*   samplers.py:233-279, diffusion.py:123-168,315-387
  *   mdm_sampler_step     samplers.py:281-345 (get_prediction_xt_last) as used by :392-433,:655-713
+ *   mdm_sampler_multistep  DPM-Solver++ 2M / 2M SDE update (Lu et al. 2022); no counterpart in the reference
  *   mdm_op_*             single fused operators, exported so parity tests can pin each kernel
  *
  * Conventions: every function returns 0 on success and a negative code on failure; the message is
@@ -415,6 +416,17 @@ int mdm_sampler_step_dynamic(const float* x_t, const float* pred, const float* n
                              int s_index, int prediction_type, const float* bound, float image_scale, int use_ddim,
                              float ddim_eta, int need_noise, float* x0_out, float* x_s_out, int batch, int64_t per_sample,
                              mdm_stream_t stream);
+/* One DPM-Solver++ multistep update (2M, or 2M SDE) of one level, in one pass:
+ *   x0_out = the data prediction of mdm_sampler_step at g = gammas[t_index], thresholded as there: clip (0/1) with
+ *            image_scale, or, when bound != NULL, the dynamic bound of mdm_dynamic_threshold (clip is then ignored);
+ *            bit-identical to mdm_sampler_step's / mdm_sampler_step_dynamic's x0_out on the same inputs
+ *   x_s_out = coef_xt * x_t + coef_x0 * x0_out + coef_x0_prev * x0_prev + coef_noise * noise
+ * The coefficients come from the caller (Sampler.multistep_coefficients). x0_prev is required when coef_x0_prev != 0,
+ * noise when coef_noise != 0; neither is read otherwise. All tensors (batch, per_sample) fp32. */
+int mdm_sampler_multistep(const float* x_t, const float* pred, const float* x0_prev, const float* noise,
+                          const float* gammas, int t_index, int prediction_type, int clip, const float* bound,
+                          float image_scale, float coef_xt, float coef_x0, float coef_x0_prev, float coef_noise,
+                          float* x0_out, float* x_s_out, int batch, int64_t per_sample, mdm_stream_t stream);
 /* classifier-free guidance: out = uncond + w * (cond - uncond)  (samplers.py:449-455) */
 int mdm_cfg_combine(const float* uncond, const float* cond, float guidance_scale, float* out, int64_t numel,
                     mdm_stream_t stream);

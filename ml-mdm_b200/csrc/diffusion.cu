@@ -142,6 +142,19 @@ __global__ void loss_bwd_kernel(const float* __restrict__ model_out, const float
   }
 }
 
+// Thresholded x0 of element k, shared by the reverse-step kernels so that they produce the same bits.
+__device__ __forceinline__ float thresholded_x0(int ptype, float x, float p, float a, float c, int clip,
+                                                float image_scale, const float* __restrict__ bound, long long k,
+                                                long long per) {
+  if (bound != nullptr) {  // dynamic thresholding (samplers.py:461-508): clamp(x0 s, -b, b) / b / s, b per sample
+    const float b = bound[k / per];
+    return __fdiv_rn(__fdiv_rn(fminf(fmaxf(x0_scaled(ptype, x, p, a, c, image_scale), -b), b), b), image_scale);
+  }
+  float x0 = x0_from_pred(ptype, x, p, a, c);
+  if (clip) x0 = fminf(fmaxf(x0 * image_scale, -1.0f), 1.0f) / image_scale;
+  return x0;
+}
+
 // One reverse step for one resolution level (samplers.py:281-345).
 //   mode 0: DDPM posterior mean (ddim_eta is None); mode 1: DDIM with eta (>= 0)
 __global__ void sampler_step_kernel(const float* __restrict__ xt, const float* __restrict__ pred,
@@ -158,14 +171,7 @@ __global__ void sampler_step_kernel(const float* __restrict__ xt, const float* _
   const long long gs = static_cast<long long>(gridDim.x) * blockDim.x;
   for (; k < total; k += gs) {
     const float x = xt[k];
-    float x0;
-    if (bound != nullptr) {  // dynamic thresholding (samplers.py:461-508): clamp(x0 s, -b, b) / b / s, b per sample
-      const float b = bound[k / per];
-      x0 = __fdiv_rn(__fdiv_rn(fminf(fmaxf(x0_scaled(ptype, x, pred[k], a, c, image_scale), -b), b), b), image_scale);
-    } else {
-      x0 = x0_from_pred(ptype, x, pred[k], a, c);
-      if (clip) x0 = fminf(fmaxf(x0 * image_scale, -1.0f), 1.0f) / image_scale;
-    }
+    const float x0 = thresholded_x0(ptype, x, pred[k], a, c, clip, image_scale, bound, k, per);
     float xs;
     float bt = beta_tilde;
     int nn = need_noise;
@@ -183,6 +189,29 @@ __global__ void sampler_step_kernel(const float* __restrict__ xt, const float* _
     }
     if (nn) xs = xs + sqrtf(bt) * noise[k];
     if (x0_out != nullptr) x0_out[k] = x0;
+    xs_out[k] = xs;
+  }
+}
+
+// One DPM-Solver++ multistep update of one level (2M, or 2M SDE with noise): x0 as sampler_step_kernel computes it,
+// then x_s = A x_t + B x0 + C x0_prev + S z with the step's coefficients from the host (C = 0: no x0_prev read;
+// S = 0: no noise read). One pass: at most four reads and two writes per element.
+__global__ void multistep_kernel(const float* __restrict__ xt, const float* __restrict__ pred,
+                                 const float* __restrict__ x0_prev, const float* __restrict__ noise,
+                                 const float* __restrict__ gammas, int t_idx, int ptype, int clip, float image_scale,
+                                 const float* __restrict__ bound, long long per, float A, float B, float Cc, float S,
+                                 float* __restrict__ x0_out, float* __restrict__ xs_out, long long total) {
+  const float g = gammas[t_idx];
+  const float a = sqrtf(g), c = sqrtf(1.0f - g);
+  long long k = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const long long gs = static_cast<long long>(gridDim.x) * blockDim.x;
+  for (; k < total; k += gs) {
+    const float x = xt[k];
+    const float x0 = thresholded_x0(ptype, x, pred[k], a, c, clip, image_scale, bound, k, per);
+    float xs = fmaf(B, x0, A * x);
+    if (x0_prev != nullptr) xs = fmaf(Cc, x0_prev[k], xs);
+    if (noise != nullptr) xs = fmaf(S, noise[k], xs);
+    x0_out[k] = x0;
     xs_out[k] = xs;
   }
 }
@@ -451,6 +480,28 @@ int mdm_sampler_step_dynamic(const float* x_t, const float* pred, const float* n
     mdm::sampler_step_kernel<<<mdm::grid_for(numel), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         x_t, pred, noise, gammas, t_index, s_index, prediction_type, 1, image_scale, use_ddim ? 1 : 0, ddim_eta,
         need_noise, x0_out, x_s_out, numel, bound, per_sample);
+    ++mdm::g_launch_count;
+    MDM_CUDA(cudaGetLastError());
+  })
+}
+
+int mdm_sampler_multistep(const float* x_t, const float* pred, const float* x0_prev, const float* noise,
+                          const float* gammas, int t_index, int prediction_type, int clip, const float* bound,
+                          float image_scale, float coef_xt, float coef_x0, float coef_x0_prev, float coef_noise,
+                          float* x0_out, float* x_s_out, int batch, int64_t per_sample, mdm_stream_t stream) {
+  MDM_TRY({
+    if (x_t == nullptr || pred == nullptr || gammas == nullptr || x0_out == nullptr || x_s_out == nullptr)
+      throw mdm::MdmFail("mdm_sampler_multistep: x_t, pred, gammas, x0_out and x_s_out are required");
+    if (batch < 1 || per_sample < 1) throw mdm::MdmFail("mdm_sampler_multistep: bad sizes");
+    if (coef_x0_prev != 0.f && x0_prev == nullptr)
+      throw mdm::MdmFail("mdm_sampler_multistep: x0_prev required for a second-order step");
+    if (coef_noise != 0.f && noise == nullptr)
+      throw mdm::MdmFail("mdm_sampler_multistep: noise tensor required for a stochastic step");
+    const long long numel = static_cast<long long>(batch) * per_sample;
+    mdm::multistep_kernel<<<mdm::grid_for(numel), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        x_t, pred, coef_x0_prev != 0.f ? x0_prev : nullptr, coef_noise != 0.f ? noise : nullptr, gammas, t_index,
+        prediction_type, clip, image_scale, bound, per_sample, coef_xt, coef_x0, coef_x0_prev, coef_noise, x0_out,
+        x_s_out, numel);
     ++mdm::g_launch_count;
     MDM_CUDA(cudaGetLastError());
   })

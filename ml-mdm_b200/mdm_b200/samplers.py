@@ -4,8 +4,9 @@
   Sampler               samplers.py:177-609   (get_eps_time, get_xt, get_xt_minus_1, forward_model,
                                                sample/_sample generator protocol, _postprocess, set_timesteps)
   NestedSampler         samplers.py:612-793   (per-resolution shifted schedules, list inputs/outputs)
+  solver=               DPM-Solver++ 2M / 2M SDE multistep sampling (no counterpart in the reference)
 
-Per-pixel algebra runs in libmdm_b200.so (mdm_q_sample / mdm_sampler_step / mdm_cfg_combine); gamma
+Per-pixel algebra runs in libmdm_b200.so (mdm_q_sample / mdm_sampler_step / mdm_sampler_multistep / mdm_cfg_combine); gamma
 is a per-sample table lookup on the device, never a (B,C,H,W) map.  Index math (time steps, table
 indices) is integer/float64 on the host exactly as in the reference.
 """
@@ -47,6 +48,46 @@ def squaredcos_cap_v2(timesteps: int) -> np.ndarray:
     for i in range(timesteps):
         betas.append(min(1 - abar((i + 1) / timesteps) / abar(i / timesteps), 0.999))
     return np.exp(np.cumsum(np.log(1.0 - np.asarray(betas))))
+
+
+SOLVERS = ("dpmpp_2m", "dpmpp_2m_sde")
+
+
+def multistep_coefficients(solver: str, gammas, t: int, s: int, h_prev=None):
+    """DPM-Solver++ (Lu et al. 2022) step t -> s of one level: (A, B, C, S, h) with
+    x_s = A x_t + B x0_t + C x0_prev + S z, in float64 from the level's gamma table.
+
+    alpha = sqrt(g), sigma = sqrt(1 - g), lambda = log alpha - log sigma, h = lambda_s - lambda_t, r = h_prev / h.
+      dpmpp_2m      A = sigma_s / sigma_t,          E = 1 - e^-h
+      dpmpp_2m_sde  A = sigma_s / sigma_t e^-h,     E = 1 - e^-2h,   S = sigma_s sqrt(E)
+    first order (no previous x0): B = alpha_s E, C = 0; second order: B = alpha_s E (1 + 1/2r), C = -alpha_s E / 2r.
+    The final step (s = 0, sigma_s = 0) returns x0: A = C = S = 0, B = 1, h = None.
+    h_prev: the level's previous h (None on its first step, or after a step of zero length)."""
+    if s == 0:
+        return 0.0, 1.0, 0.0, 0.0, None
+    g_t, g_s = float(gammas[t]), float(gammas[s])
+    a_t, a_s = math.sqrt(g_t), math.sqrt(g_s)
+    sig_t, sig_s = math.sqrt(1.0 - g_t), math.sqrt(1.0 - g_s)
+    h = (math.log(a_s) - math.log(sig_s)) - (math.log(a_t) - math.log(sig_t))
+    if solver == "dpmpp_2m_sde":
+        A, E = sig_s / sig_t * math.exp(-h), -math.expm1(-2.0 * h)
+        S = sig_s * math.sqrt(E)
+    else:
+        A, E, S = sig_s / sig_t, -math.expm1(-h), 0.0
+    B, Cc = a_s * E, 0.0
+    if h_prev:
+        half_inv_r = h / (2.0 * h_prev)
+        B, Cc = a_s * E * (1.0 + half_inv_r), -a_s * E * half_inv_r
+    return A, B, Cc, S, h
+
+
+def check_solver(solver, ddim_eta):
+    if solver is None:
+        return
+    if solver not in SOLVERS:
+        raise ValueError(f"unknown solver {solver!r}: expected None or one of {SOLVERS}")
+    if ddim_eta is not None:
+        raise ValueError(f"solver={solver!r} does not take ddim_eta (got {ddim_eta!r})")
 
 
 def _stream():
@@ -212,6 +253,38 @@ class Sampler(nn.Module):
                                                C.c_int64(x_t.numel()), _stream()), "mdm_sampler_step")
         return x0, x_s
 
+    def _multistep_level(self, x_t, pred, t_idx, s_idx, scale, image_scale, solver, hist):
+        """One DPM-Solver++ step of one level (mdm_sampler_multistep): x0 thresholded as _step_level does, then
+        x_s = A x_t + B x0 + C x0_prev (+ S z). hist: the level's (x0, h) of its previous step, or None.
+        Returns (x0, x_s, the level's new hist)."""
+        x_t, pred = _f32c(x_t), _f32c(pred)
+        tab = self.level_table(scale, x_t.device)
+        x0_prev, h_prev = hist if hist is not None else (None, None)
+        A, Bc, Cc, S, h = multistep_coefficients(solver, self.level_table(scale, "cpu"), t_idx, s_idx, h_prev)
+        noise = torch.randn_like(x_t) if S != 0.0 else None
+        ptype = self._config.prediction_type.value
+        clip = self._clip_flag()
+        bound = self._dynamic_bound(x_t, pred, tab, t_idx, ptype, image_scale) if clip == 2 else None
+        x0 = torch.empty_like(x_t)
+        x_s = torch.empty_like(x_t)
+        B = x_t.shape[0]
+        _lib.check(_lib.lib().mdm_sampler_multistep(_ptr(x_t), _ptr(pred), _ptr(x0_prev), _ptr(noise), _ptr(tab),
+                                                    int(t_idx), int(ptype), clip, _ptr(bound), C.c_float(image_scale),
+                                                    C.c_float(A), C.c_float(Bc), C.c_float(Cc), C.c_float(S),
+                                                    _ptr(x0), _ptr(x_s), B, C.c_int64(x_t.numel() // B), _stream()),
+                   "mdm_sampler_multistep")
+        return x0, x_s, (x0, h)
+
+    def _solver_step(self, model, t, s, x_t, lm_outputs, lm_mask, micros, guidance_scale, solver, hist):
+        """One DPM-Solver++ step t -> s (the model sees t - 1). hist: per level index, the level's previous (x0, h);
+        updated in place. Returns (x0, x_s, (gamma_t, gamma_s)) as get_xt_minus_1(return_details=True) does."""
+        B = x_t.shape[0]
+        times = torch.full((B,), t - 1, dtype=torch.long, device=x_t.device)
+        pred, _ = self.forward_model(model, x_t, times, lm_outputs, lm_mask, micros, guidance_scale)
+        rs = self._config.rescale_signal
+        x0, x_s, hist[0] = self._multistep_level(x_t, pred, t, s, 1.0, 1.0 if rs is None else rs, solver, hist.get(0))
+        return x0, x_s, (self.gammas[t], self.gammas[s])
+
     def get_xt_minus_1(self, model, time_step, x_t, lm_outputs, lm_mask, micros={}, time_step_last=None,
                        guidance_scale: float = 1, ddim_eta=None, return_details: bool = False):
         """One reverse step (samplers.py:392-433). The model sees t-1."""
@@ -316,9 +389,11 @@ class Sampler(nn.Module):
     def _sample(self, model, x_t, lm_outputs, lm_mask, micros, return_sequence: bool = False,
                 use_beta_tilde: bool = False, t: int = -1, num_inference_steps: int = 2000, ddim_eta=None,
                 guidance_scale: float = 1, resample_steps: bool = False, disable_bar: bool = True,
-                yield_output: bool = False, **post_args):
-        """p_sample loop (samplers.py:516-578), generator protocol preserved."""
+                yield_output: bool = False, solver=None, **post_args):
+        """p_sample loop (samplers.py:516-578), generator protocol preserved.
+        solver: None (DDPM, or DDIM with ddim_eta) or one of SOLVERS, DPM-Solver++ multistep over the same time steps."""
         assert not (yield_output and return_sequence), "not allowed."
+        check_solver(solver, ddim_eta)
         if not resample_steps:
             num_inference_steps = self.n_steps
         timesteps = self.set_timesteps(num_inference_steps)
@@ -326,15 +401,20 @@ class Sampler(nn.Module):
             timesteps = timesteps[timesteps <= t]
         seq = [x_t] if return_sequence else []
         x0, extra = None, None
+        hist = {}
         with torch.no_grad():
             self._text = self._encode_text(model, lm_outputs, lm_mask)
             try:
                 for i, tt in enumerate(timesteps[:-1]):
                     t_last = timesteps[i + 1] if resample_steps else None
-                    x0, x_t, extra = self.get_xt_minus_1(model, int(tt), x_t, lm_outputs, lm_mask, micros,
-                                                         time_step_last=None if t_last is None else int(t_last),
-                                                         guidance_scale=guidance_scale, ddim_eta=ddim_eta,
-                                                         return_details=True)
+                    if solver is not None:
+                        x0, x_t, extra = self._solver_step(model, int(tt), int(timesteps[i + 1]), x_t, lm_outputs,
+                                                           lm_mask, micros, guidance_scale, solver, hist)
+                    else:
+                        x0, x_t, extra = self.get_xt_minus_1(model, int(tt), x_t, lm_outputs, lm_mask, micros,
+                                                             time_step_last=None if t_last is None else int(t_last),
+                                                             guidance_scale=guidance_scale, ddim_eta=ddim_eta,
+                                                             return_details=True)
                     if yield_output:
                         yield self._postprocess(x_t, x0, extra, **post_args)
                     if return_sequence:
@@ -385,13 +465,7 @@ class NestedSampler(Sampler):
                        guidance_scale=1, ddim_eta=None, return_details=False):
         """samplers.py:655-713. x_t: full-resolution tensor (first call) or list high -> low."""
         scales = model.vision_model.nest_ratio + [1]
-        if isinstance(x_t, torch.Tensor):
-            out = [x_t]
-            for s in scales[1:]:
-                ratio = scales[0] // s
-                b, c, h, w = x_t.shape
-                out.append(torch.empty(b, c, h // ratio, w // ratio, device=x_t.device, dtype=x_t.dtype).normal_())
-            x_t = out
+        x_t = self._level_inputs(x_t, scales)
         t = int(time_step)
         s_idx = t - 1 if time_step_last is None else int(time_step_last)
         B = x_t[0].shape[0]
@@ -407,6 +481,35 @@ class NestedSampler(Sampler):
             tab = self.level_table(scales[-1], x_t[0].device)
             return x0, x_s, (tab[t], tab[s_idx])
         return x_s
+
+    @staticmethod
+    def _level_inputs(x_t, scales):
+        """The first step's full-resolution tensor -> one tensor per level, the lower ones drawn with normal_
+        (samplers.py:664-672); a list is returned as it is."""
+        if not isinstance(x_t, torch.Tensor):
+            return x_t
+        out = [x_t]
+        for s in scales[1:]:
+            ratio = scales[0] // s
+            b, c, h, w = x_t.shape
+            out.append(torch.empty(b, c, h // ratio, w // ratio, device=x_t.device, dtype=x_t.dtype).normal_())
+        return out
+
+    def _solver_step(self, model, t, s, x_t, lm_outputs, lm_mask, micros, guidance_scale, solver, hist):
+        """Sampler._solver_step per level, each with its own table and history (x_t as in get_xt_minus_1)."""
+        scales = model.vision_model.nest_ratio + [1]
+        x_t = self._level_inputs(x_t, scales)
+        B = x_t[0].shape[0]
+        times = torch.full((B,), t - 1, dtype=torch.long, device=x_t[0].device)
+        p_t = self.forward_model(model, x_t, times, lm_outputs, lm_mask, micros, guidance_scale)
+        x0, x_s = [], []
+        for l, (x, p, sc) in enumerate(zip(x_t, p_t, scales)):
+            a, b, hist[l] = self._multistep_level(x, p, t, s, sc, 1.0 if self._config.schedule_shifted else float(sc),
+                                                  solver, hist.get(l))
+            x0.append(a)
+            x_s.append(b)
+        tab = self.level_table(scales[-1], x_t[0].device)
+        return x0, x_s, (tab[t], tab[s])
 
     def _postprocess(self, x_t, x0=None, extra=None, yield_full: bool = False, clip: bool = False,
                      output_inner: bool = False, **unused):
