@@ -3,11 +3,11 @@ import os, sys, copy
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE); sys.path.insert(0, os.path.join(HERE, "..")); sys.path.insert(0, os.path.join(HERE, "..", "ml-mdm_b200"))
 import torch
-import net_cases as nc
+import parity
 import tiny_configs as tc
 
 def grads(kind, steps=3):
-    model, _, _ = nc.build(kind)
+    model, _, _ = parity.tiny_model(tc.TINY[kind])
     model = model.cuda()
     nlev = 1 if kind == "unet" else 2
     out = []

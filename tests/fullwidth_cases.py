@@ -23,6 +23,7 @@ for p in (HERE, os.path.join(HERE, ".."), os.path.join(HERE, "..", "ml-mdm_b200"
     if p not in sys.path:
         sys.path.insert(0, p)
 
+import parity  # noqa: E402
 from mdm_b200 import config as mc  # noqa: E402
 from mdm_b200.models import NestedUNet, UNet  # noqa: E402
 from oracle import unet_ref  # noqa: E402
@@ -31,12 +32,12 @@ RES = {"cc12m_64x64": [64], "cc12m_256x256": [256, 64], "cc12m_1024x1024": [1024
 CFG_DIR = os.path.join(HERE, "..", "ml-mdm_b200", "mdm_b200", "configs")
 
 
-def rel(a, b):
-    return float((a.double() - b.double()).abs().max() / b.double().abs().max().clamp_min(1e-300))
-
-
-def build(name, seed=0):
+def build(name, seed=0, edit=None):
+    """(the model of configs/<name>.yaml, its config for the oracle). edit(config), when given, changes the loaded
+    config before the model is built, e.g. to add lm_head layers or dropout."""
     ucfg, _, nested = mc.load_yaml_configs(os.path.join(CFG_DIR, name + ".yaml"))
+    if edit is not None:
+        edit(ucfg)
     ocfg = copy.deepcopy(ucfg)
     torch.manual_seed(seed)
     m = (NestedUNet if nested else UNet)(3, 3, ucfg)
@@ -44,7 +45,7 @@ def build(name, seed=0):
         for p in m.parameters():
             if float(p.abs().max()) == 0:
                 p.normal_(0, 0.02)
-    return m, ocfg, nested
+    return m, ocfg
 
 
 def inputs(name, B, S, seed=1, ragged=True, micro=False):
@@ -65,72 +66,34 @@ def inputs(name, B, S, seed=1, ragged=True, micro=False):
     return xs, t, lm, mask, ws, micros
 
 
-def run_oracle(ocfg, sd, xs, t, lm, mask, ws, micros, dtype, tf32):
-    dev = "cuda"
-    torch.backends.cuda.matmul.allow_tf32 = bool(tf32)
-    torch.backends.cudnn.allow_tf32 = bool(tf32)
-    try:
-        net = unet_ref.OracleNet(ocfg, 2048)
-        P = {k: v.to(dev, dtype).requires_grad_(True) for k, v in sd.items()}
-        nested = len(xs) > 1
-        xin = [x.to(dev, dtype) for x in xs]
-        mic = {k: v.to(dev) for k, v in micros.items()}
-        out = net.forward(P, xin if nested else xin[0], t.to(dev), lm.to(dev, dtype), mask.to(dev, dtype), mic)
-        outs = list(out) if nested else [out]
-        loss = sum((o * w.to(dev, dtype)).sum() for o, w in zip(outs, ws))
-        loss.backward()
-        torch.cuda.synchronize()
-        res = ([o.detach().cpu() for o in outs], {k: P[k].grad.detach().cpu() for k in P if P[k].grad is not None})
-    finally:
-        torch.backends.cuda.matmul.allow_tf32 = False
-        torch.backends.cudnn.allow_tf32 = False
-    del P, out, outs, loss
-    torch.cuda.empty_cache()
-    return res
-
-
-def run_ours(m, xs, t, lm, mask, ws, micros):
-    m = m.cuda()
-    nested = len(xs) > 1
-    xin = [x.cuda() for x in xs]
-    mic = {k: v.cuda() for k, v in micros.items()}
-    out = m(xin if nested else xin[0], t.cuda(), lm.cuda(), mask.cuda(), mic)
-    outs = list(out) if nested else [out]
-    loss = sum((o * w.cuda()).sum() for o, w in zip(outs, ws))
-    loss.backward()
-    torch.cuda.synchronize()
-    return [o.detach().cpu() for o in outs], {k: p.grad.detach().cpu() for k, p in m.named_parameters() if p.grad is not None}
-
-
-def run_case(name, B=1, S=8, micro=False, verbose=False):
-    """Returns {"out": [(ours, tf32), ...], "grads": {param: (ours, tf32)}, "seconds": {...}}."""
-    m, ocfg, nested = build(name)
+def run_case(name, m, oracle, B=1, S=8, micro=False, micros=None, verbose=False):
+    """The engine `m`, `oracle` in float64 and the oracle in float32 with TF32 on, all on the GPU, with inputs(name, B,
+    S, micro=micro) (micros, when given, in place of its micro-conditioning values). Returns parity.report(...,
+    floor=False) with "seconds" per arm and the extras of parity.assert_calibrated_full_width."""
     sd = {k: v.detach().clone() for k, v in m.state_dict().items()}
-    xs, t, lm, mask, ws, micros = inputs(name, B, S, micro=micro)
+    xs, t, lm, mask, ws, mic = inputs(name, B, S, micro=micro)
+    args = (sd, xs, t, lm, mask, mic if micros is None else micros, ws)
     tm = {}
     t0 = time.time()
-    o64, g64 = run_oracle(ocfg, sd, xs, t, lm, mask, ws, micros, torch.float64, False)
+    o64, g64 = parity.oracle_arm(oracle.forward, *args, torch.float64, "cuda")
     tm["f64"] = time.time() - t0
     t0 = time.time()
-    o32, g32 = run_oracle(ocfg, sd, xs, t, lm, mask, ws, micros, torch.float32, True)
+    o32, g32 = parity.oracle_arm(oracle.forward, *args, torch.float32, "cuda", tf32=True)
     tm["tf32"] = time.time() - t0
     t0 = time.time()
-    oo, go = run_ours(m, xs, t, lm, mask, ws, micros)
+    oo, go = parity.engine_arm(m, xs, *args[2:])
     tm["ours"] = time.time() - t0
-    rep = {"out": [(rel(a, r), rel(b, r)) for a, b, r in zip(oo, o32, o64)], "grads": {}, "seconds": tm,
-           "missing": [k for k in g64 if k not in go]}
+    rep = parity.report((oo, go), (o64, g64), (o32, g32), floor=False)
+    rep["seconds"] = tm
     rep["grad_absmax"] = {k: float(go[k].abs().max()) for k in go}
     rep["grad_absmax_tf32"] = {k: float(g32[k].abs().max()) for k in g32}
     mags = sorted(float(r.abs().max()) for r in g64.values())
     rep["grad_typical"] = mags[len(mags) // 2]  # median over parameters of max|d loss / d parameter|
-    for k, r in g64.items():
-        if k in go:
-            rep["grads"][k] = (rel(go[k], r), rel(g32[k], r))
     if verbose:
         print(f"== {name} B={B} S={S} micro={micro}: seconds {tm}")
         for i, (a, b) in enumerate(rep["out"]):
             print(f"   out[{i}]  ours {a:.3e}   reference-tf32 {b:.3e}")
-        defined = {k: v for k, v in rep["grads"].items() if v[1] <= 0.5}
+        defined = parity.defined_grads(rep["grads"])
         print(f"   numerically undefined gradients (reference-tf32 error > 0.5, mathematically zero): "
               f"{sorted(k for k in rep['grads'] if k not in defined)}")
         ge = sorted(defined.items(), key=lambda kv: -kv[1][0])
@@ -159,7 +122,9 @@ if __name__ == "__main__":
 
         buf = io.StringIO()
         with contextlib.redirect_stdout(buf):
-            run_case(nm, B=2 if nm != "cc12m_1024x1024" else 1, S=8, micro=True, verbose=True)
+            m, ocfg = build(nm)
+            run_case(nm, m, unet_ref.OracleNet(ocfg, 2048), B=2 if nm != "cc12m_1024x1024" else 1, S=8, micro=True,
+                     verbose=True)
         print(buf.getvalue(), flush=True)
         with open(os.path.join(HERE, "..", "gpurun_out", f"parity_fullwidth_{nm}.txt"), "w") as f:
             f.write(buf.getvalue())

@@ -1,9 +1,7 @@
 """Parity of the native (nested) U-Net against the oracle on tiny configs: forward, intermediate
 activations and every parameter gradient.  Used by tests/test_net_gpu.py; runnable as a script."""
-import copy
 import os
 import sys
-import types
 
 import torch
 
@@ -12,126 +10,51 @@ sys.path.insert(0, HERE)
 sys.path.insert(0, os.path.join(HERE, ".."))
 sys.path.insert(0, os.path.join(HERE, "..", "ml-mdm_b200"))
 
+import parity  # noqa: E402
 import tiny_configs as tc  # noqa: E402
-from mdm_b200 import config as mc  # noqa: E402
-from mdm_b200.models import NestedUNet, UNet  # noqa: E402
-from oracle import unet_ref  # noqa: E402
+from parity import assert_calibrated  # noqa: E402,F401  (the bounds run_case's report is held to)
 
 
-def rel(a, b):
-    return float((a - b).abs().max() / b.abs().max().clamp_min(1e-30))
-
-
-def build(kind, seed=7):
-    ucfg = copy.deepcopy(tc.TINY_UNET if kind == "unet" else tc.TINY_NESTED)
-    cfg = mc.unet_config_from_dict(ucfg)
-    cfg.conditioning_feature_dim = tc.LM_DIM
-    ocfg = copy.deepcopy(cfg)  # the model constructor mutates conditioning_feature_dim
-    model = (UNet if kind == "unet" else NestedUNet)(3, 3, cfg)
-    sd = tc.seeded_state_dict(model.state_dict(), seed)
-    model.load_state_dict(sd)
-    oracle = unet_ref.OracleNet(ocfg, tc.LM_DIM)
-    return model, oracle, sd
-
-
-def run_case(kind, batch=2, tokens=6, dtype=torch.float64, verbose=True, res=None):
+def run_case(kind, built=None, inputs=None, acts=True, verbose=True):
+    """Forward + backward of loss = sum_l <out_l, w_l> on the engine, the fp64 oracle (CPU) and the reference-TF32 arm
+    (the oracle in fp32 on the GPU with TF32 on): parity.report, and with acts the error of every residual-stream
+    activation the fp64 oracle traces ("acts"). built: (model, oracle, state_dict), by default parity.tiny_model of
+    the kind's tiny config; inputs: (x, t, lm, mask), by default tc.seeded_inputs(3, ...) at batch 2 and 6 tokens."""
     nlev = 1 if kind == "unet" else 2
-    res = res or (16 if kind == "unet" else 32)
-    model, oracle, sd = build(kind)
-    x, t, lm, mask = tc.seeded_inputs(3, batch, res, tokens, nlevels=nlev)
+    model, oracle, sd = built or parity.tiny_model(tc.TINY[kind])
+    x, t, lm, mask = inputs or tc.seeded_inputs(3, 2, 16 if kind == "unet" else 32, 6, nlevels=nlev)
     xs = [x] if nlev == 1 else x
     g = torch.Generator().manual_seed(11)
     ws = [torch.randn(xi.shape, generator=g) for xi in xs]
-
-    # ---- oracle (CPU, fp64 by default: arbitrates between two fp32-ish implementations)
-    P = {k: v.to(dtype).requires_grad_(True) for k, v in sd.items()}
     trace = {}
-    o_out = oracle.forward(P, [xi.to(dtype) for xi in xs] if nlev > 1 else xs[0].to(dtype), t, lm.to(dtype),
-                           mask.to(dtype), {}, trace=trace)
-    o_outs = [o_out] if nlev == 1 else list(o_out)
-    loss = sum((o * w.to(dtype)).sum() for o, w in zip(o_outs, ws))
-    loss.backward()
-
-    # ---- native
-    model = model.cuda()
-    xs_c = [xi.cuda() for xi in xs]
-    out = model(xs_c if nlev > 1 else xs_c[0], t.cuda(), lm.cuda(), mask.cuda(), {})
-    outs = [out] if nlev == 1 else list(out)
-    nloss = sum((o * w.cuda()).sum() for o, w in zip(outs, ws))
-    nloss.backward()
-    torch.cuda.synchronize()
-
-    report = {"out": [rel(o.detach().cpu().to(dtype), r.detach()) for o, r in zip(outs, o_outs)]}
-    # calibration: the same oracle in fp32 on the GPU with TF32 enabled = the arithmetic the reference trains with
-    # (clis/train_parallel.py:18-19); its error against the fp64 oracle, measured with the same metric
-    torch.backends.cuda.matmul.allow_tf32 = True
-    torch.backends.cudnn.allow_tf32 = True
-    try:
-        Pt = {k: v.float().cuda().requires_grad_(True) for k, v in sd.items()}
-        t_out = oracle.forward(Pt, [xi.cuda() for xi in xs] if nlev > 1 else xs[0].cuda(), t.cuda(), lm.cuda(), mask.cuda(), {})
-        t_outs = [t_out] if nlev == 1 else list(t_out)
-        sum((o * w.cuda()).sum() for o, w in zip(t_outs, ws)).backward()
-        torch.cuda.synchronize()
-    finally:
-        torch.backends.cuda.matmul.allow_tf32 = False
-        torch.backends.cudnn.allow_tf32 = False
-    report["tf32_out"] = [rel(o.detach().cpu().to(dtype), r.detach()) for o, r in zip(t_outs, o_outs)]
-    # intermediates
-    acts = {}
-    for name, ref in trace.items():
-        try:
-            b, c, h, w = ref.shape
-            got = model.native().debug_fetch(name, (b, h, w, c)).permute(0, 3, 1, 2).cpu().to(dtype)
-            acts[name] = rel(got, ref.detach())
-        except Exception as e:  # intermediates are released in inference mode only; report and go on
-            acts[name] = str(e)
-    report["acts"] = acts
-    grads = {}
-    # Gradients that are mathematically zero (a conv bias feeding a GroupNorm whose groups are single
-    # channels) come out as round-off on both sides: errors are measured against
-    # max(|ref_k|, 1e-2 * median_k max|ref_k|) so those are judged on the scale of real gradients.
-    mags = sorted(float(P[k].grad.abs().max()) for k, _ in model.named_parameters())
-    floor = 1e-2 * mags[len(mags) // 2]
-    for k, p in model.named_parameters():
-        ref = P[k].grad
-        if p.grad is None:
-            grads[k] = float("nan")
-            continue
-        got = p.grad.detach().cpu().to(dtype)
-        grads[k] = float((got - ref).abs().max() / max(float(ref.abs().max()), floor))
-        report.setdefault("tf32_grads", {})[k] = float((Pt[k].grad.detach().cpu().to(dtype) - ref).abs().max()
-                                                       / max(float(ref.abs().max()), floor))
-        if verbose and not (grads[k] <= 5e-2):
-            print("   BAD", k, "got", p.grad.detach().flatten()[:6].tolist(), "ref", ref.flatten()[:6].tolist())
-    report["grads"] = grads
+    f64 = parity.oracle_arm(oracle.forward, sd, xs, t, lm, mask, {}, ws, torch.float64, "cpu", trace=trace)
+    ours = parity.engine_arm(model, xs, t, lm, mask, {}, ws)
+    tf32 = parity.oracle_arm(oracle.forward, sd, xs, t, lm, mask, {}, ws, torch.float32, "cuda", tf32=True)
+    report = parity.report(ours, f64, tf32)
+    if acts:
+        report["acts"] = {}
+        for name, ref in trace.items():
+            try:
+                b, c, h, w = ref.shape
+                got = model.native().debug_fetch(name, (b, h, w, c)).permute(0, 3, 1, 2)
+                report["acts"][name] = parity.rel(got.cpu(), ref.detach())
+            except Exception as e:  # intermediates are released in inference mode only; report and go on
+                report["acts"][name] = str(e)
     if verbose:
-        print(f"== {kind}: out rel err {report['out']}  (reference-tf32: {report['tf32_out']})")
-        tg = sorted(report["tf32_grads"].values())
-        og = sorted(grads.values())
+        grads = report["grads"]
+        print(f"== {kind}: out rel err (ours, reference-tf32) {report['out']}")
+        og = sorted(v[0] for v in grads.values())
+        tg = sorted(v[1] for v in grads.values())
         print(f"   grads: ours median {og[len(og) // 2]:.2e} max {og[-1]:.2e} | reference-tf32 median {tg[len(tg) // 2]:.2e} "
               f"max {tg[-1]:.2e}")
-        bad_a = {k: v for k, v in acts.items() if isinstance(v, str) or v > 2e-3}
-        print(f"   activations checked: {len(acts)}, above 2e-3: {bad_a}")
-        worst = sorted(grads.items(), key=lambda kv: -(kv[1] if kv[1] == kv[1] else 1e9))[:12]
-        print("   worst grads (ours, reference-tf32):", [(k, f"{v:.2e}", f"{report['tf32_grads'][k]:.2e}") for k, v in worst])
-        print(f"   grads above 5e-3: {sum(1 for v in grads.values() if not (v <= 5e-3))} / {len(grads)}")
+        bad_a = {k: v for k, v in report.get("acts", {}).items() if isinstance(v, str) or v > 2e-3}
+        print(f"   activations checked: {len(report.get('acts', {}))}, above 2e-3: {bad_a}")
+        worst = sorted(grads.items(), key=lambda kv: -(kv[1][0] if kv[1][0] == kv[1][0] else 1e9))[:12]
+        print("   worst grads (ours, reference-tf32):", [(k, f"{a:.2e}", f"{b:.2e}") for k, (a, b) in worst])
+        print(f"   grads above 5e-3: {sum(1 for v in og if not (v <= 5e-3))} / {len(og)}")
+        print(f"   missing gradients: {report['missing']}")
         print("   pool bytes (reserved, high-water):", model.native().workspace_bytes())
     return report
-
-
-def assert_calibrated(r):
-    """Bounds against the reference-TF32 errors measured in the same run (see tests/test_net_gpu.py)."""
-    for ours, tf32 in zip(r["out"], r["tf32_out"]):
-        assert ours <= max(1e-3, 1.75 * tf32), (r["out"], r["tf32_out"])
-    act_lim = max(2e-3, 2.0 * max(r["tf32_out"]))
-    bad = {k: v for k, v in r["acts"].items() if isinstance(v, str) or v > act_lim}
-    assert not bad, (bad, act_lim)
-    t = sorted(r["tf32_grads"].values())
-    o = sorted(r["grads"].values())
-    med = t[len(t) // 2]
-    assert o[len(o) // 2] <= 1.5 * med, (o[len(o) // 2], med)
-    badg = {k: (v, r["tf32_grads"][k]) for k, v in r["grads"].items() if not (v <= 3.5 * max(r["tf32_grads"][k], med))}
-    assert not badg, badg
 
 
 if __name__ == "__main__":

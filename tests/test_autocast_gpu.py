@@ -11,7 +11,7 @@ autocast region multiplies the weights' hi fp16 plane only, and every other call
 
 Forward outputs are compared to 1e-6 relative (plus ten times the spread of two runs of the same call): GroupNorm
 statistics are summed by fp32 atomics, so two runs of one forward can differ in the last bits, while a pass that read a
-stale or missing lo plane is off by more than 1e-5 (asserted). Gradients: the run-to-run bound of tests/test_cond_split_gpu.py
+stale or missing lo plane is off by more than 1e-5 (asserted). Gradients: the run-to-run bound of tests/parity.py
 (weight-gradient split-K and attention dQ accumulate with fp32 atomics)."""
 import argparse
 import copy
@@ -31,17 +31,15 @@ for p in (HERE, os.path.join(HERE, ".."), os.path.join(HERE, "..", "ml-mdm_b200"
 
 import lm_head_oracle  # noqa: E402
 import micro_cases as mcases  # noqa: E402
-import net_cases as nc  # noqa: E402
+import parity  # noqa: E402
 import tiny_configs as tc  # noqa: E402
 from mdm_b200 import _lib, optim, trainer  # noqa: E402
 from mdm_b200 import config as mc  # noqa: E402
 from mdm_b200.diffusion import NestedDiffusion, NestedModel  # noqa: E402
-from mdm_b200.models import NestedUNet, UNet  # noqa: E402
 from mdm_b200.samplers import NestedSampler  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
-RUN_OUT, RUN_GRAD = 3e-3, 2e-2  # two engine runs (tests/test_cond_split_gpu.py)
 DTYPES = {"bf16": torch.bfloat16, "fp16": torch.float16}
 
 
@@ -54,14 +52,8 @@ def ucfg_of(kind):
     return u
 
 
-def build(kind, seed=7):
-    cfg = mc.unet_config_from_dict(ucfg_of(kind))
-    cfg.conditioning_feature_dim = tc.LM_DIM
-    ocfg = copy.deepcopy(cfg)  # the model constructor mutates conditioning_feature_dim
-    model = (UNet if kind == "unet" else NestedUNet)(3, 3, cfg)
-    sd = tc.seeded_state_dict(model.state_dict(), seed)
-    model.load_state_dict(sd)
-    return model, ocfg, sd
+def build(kind):
+    return parity.tiny_model(ucfg_of(kind), lm_head_oracle.OracleNet)
 
 
 def inputs(kind, batch=2):
@@ -103,16 +95,7 @@ def step(model, ins, ws, autocast=None):
 def close_out(a, b, spread):
     bound = 1e-6 + 10.0 * spread
     for x, y in zip(a, b):
-        assert nc.rel(x, y) <= bound, (nc.rel(x, y), bound)
-
-
-def close_grads(a, b):
-    mags = sorted(float(v.abs().max()) for v in b.values())
-    floor = 1e-2 * mags[len(mags) // 2]
-    assert a.keys() == b.keys()
-    for k in b:
-        e = float((a[k] - b[k]).abs().max()) / max(float(b[k].abs().max()), floor)
-        assert e <= RUN_GRAD, (k, e)
+        assert parity.rel(x, y) <= bound, (parity.rel(x, y), bound)
 
 
 def profiled(fn):
@@ -135,44 +118,16 @@ def profiled(fn):
 
 
 # ---------------------------------------------------------------- 1. calibrated accuracy
-def _oracle(ocfg, sd, ins, ws, autocast):
-    xs, t, lm, mask, micros = ins
-    net = lm_head_oracle.OracleNet(ocfg, tc.LM_DIM)
-    dt = torch.float64 if autocast is None else torch.float32
-    dev = "cpu" if autocast is None else "cuda"
-    P = {k: v.to(dev, dt).requires_grad_(True) for k, v in sd.items()}
-    xin = [x.to(dev, dt) for x in xs]
-    args = (P, xin if len(xs) > 1 else xin[0], t.to(dev), lm.to(dev, dt), mask.to(dev, dt),
-            {k: v.to(dev, dt) for k, v in micros.items()})
-    if autocast is None:
-        out = net.forward(*args)
-    else:
-        with torch.autocast("cuda", dtype=autocast):
-            out = net.forward(*args)
-    outs = list(out) if len(xs) > 1 else [out]
-    sum((o.to(dt) * w.to(dev, dt)).sum() for o, w in zip(outs, ws)).backward()
-    return [o.detach().double().cpu() for o in outs], {k: v.grad.double().cpu() for k, v in P.items() if v.grad is not None}
-
-
 def accuracy_report(kind, dtype):
-    """Errors against the fp64 oracle of the engine under autocast and of the oracle in fp32 under the same autocast:
-    {"out": [(ours, reference)], "grads": {name: (ours, reference)}, "missing": [...]}."""
-    model, ocfg, sd = build(kind)
-    ins = inputs(kind)
-    ws = [w.cpu() for w in weights(ins[0])]
-    o64, g64 = _oracle(ocfg, sd, ins, ws, None)
-    oac, gac = _oracle(ocfg, sd, ins, ws, DTYPES[dtype])
-    model = model.cuda()
-    outs, grads = step(model, cuda_all(*ins), [w.cuda() for w in ws], DTYPES[dtype])
-    rep = {"out": [(nc.rel(a.cpu().double(), r), nc.rel(b, r)) for a, b, r in zip(outs, oac, o64)], "grads": {},
-           "missing": sorted(k for k in g64 if k not in grads)}
-    mags = sorted(float(r.abs().max()) for r in g64.values())
-    floor = 1e-2 * mags[len(mags) // 2]
-    for k, r in g64.items():
-        if k in grads:
-            d = max(float(r.abs().max()), floor)
-            rep["grads"][k] = (float((grads[k].cpu().double() - r).abs().max()) / d, float((gac[k] - r).abs().max()) / d)
-    return rep
+    """Errors against the fp64 oracle (CPU) of the engine under autocast and of the oracle in fp32 under the same
+    autocast: parity.report."""
+    model, oracle, sd = build(kind)
+    xs, t, lm, mask, micros = inputs(kind)
+    ws = [w.cpu() for w in weights(xs)]
+    args = (sd, xs, t, lm, mask, micros, ws)
+    return parity.report(parity.engine_arm(model, xs, t, lm, mask, micros, ws, autocast=DTYPES[dtype]),
+                         parity.oracle_arm(oracle.forward, *args, torch.float64, "cpu"),
+                         parity.oracle_arm(oracle.forward, *args, torch.float32, "cuda", autocast=DTYPES[dtype]))
 
 
 @pytest.mark.parametrize("dtype", list(DTYPES))
@@ -180,7 +135,7 @@ def accuracy_report(kind, dtype):
 def test_autocast_within_the_reference_autocast_error(kind, dtype):
     rep = accuracy_report(kind, dtype)
     # the bounds of the fp32 path (DESIGN.md section 4), with the reference's autocast error in place of its TF32 one
-    mcases.assert_calibrated(rep)
+    parity.assert_calibrated(rep)
 
 
 # ---------------------------------------------------------------- 2. the path really changed
@@ -221,11 +176,11 @@ def test_fp32_after_autocast_and_weight_update_matches_a_fresh_net(graphs):
         oa, ga = step(a, ins, ws)
         ob, gb = step(b, ins, ws)
     ob2, _ = step(b, ins, ws)
-    close_out(oa, ob, max(nc.rel(x, y) for x, y in zip(ob2, ob)))
-    close_grads(ga, gb)
+    close_out(oa, ob, max(parity.rel(x, y) for x, y in zip(ob2, ob)))
+    parity.assert_same_run([], [], ga, gb)
     # what the comparison guards: a single-plane result is far outside that bound
     ob_ac, _ = step(b, ins, ws, torch.bfloat16)
-    assert min(nc.rel(x, y) for x, y in zip(ob_ac, ob)) > 1e-5
+    assert min(parity.rel(x, y) for x, y in zip(ob_ac, ob)) > 1e-5
 
 
 # ---------------------------------------------------------------- 4. graphs alternating between the modes
@@ -243,8 +198,8 @@ def test_graph_replay_alternating_modes_matches_eager():
         og, gg = step(graph, ins, ws, ac)
         oe, ge = step(eager, ins, ws, ac)
         oe2, _ = step(eager, ins, ws, ac)
-        close_out(og, oe, max(nc.rel(x, y) for x, y in zip(oe2, oe)))
-        close_grads(gg, ge)
+        close_out(og, oe, max(parity.rel(x, y) for x, y in zip(oe2, oe)))
+        parity.assert_same_run([], [], gg, ge)
         with torch.no_grad():  # the same in-place update on both
             for pg, pe in zip(graph.parameters(), eager.parameters()):
                 d = 1e-3 * torch.sin(pg * (i + 1))
@@ -277,8 +232,8 @@ def test_cond_cache_across_a_mode_change():
             o2 = model.forward_denoising(xs, t, *enc, micros)
             ref = model(xs, t, lm, mask, micros)
         assert nat._cache_mode(xs, enc[1], enc[2]) == 1  # back outside autocast: the single-plane fill is not reused
-    for a, b, r in zip(o1, o2, ref):
-        assert nc.rel(a, r) <= RUN_OUT and nc.rel(b, r) <= RUN_OUT
+    parity.assert_same_run(o1, ref)
+    parity.assert_same_run(o2, ref)
 
 
 def test_ddim_under_autocast_with_text_encoded_once_matches_per_step():
@@ -305,7 +260,7 @@ def test_ddim_under_autocast_with_text_encoded_once_matches_per_step():
     a = run(False)
     b = run(True)
     b2 = run(True)
-    assert nc.rel(a, b) <= max(RUN_OUT, 3.0 * nc.rel(b2, b)), (nc.rel(a, b), nc.rel(b2, b))
+    assert parity.rel(a, b) <= max(parity.RUN_OUT, 3.0 * parity.rel(b2, b)), (parity.rel(a, b), parity.rel(b2, b))
 
 
 # ---------------------------------------------------------------- 6. train_batch with args.fp16
@@ -351,6 +306,6 @@ def test_train_batch_fp16_runs_single_plane_and_matches_explicit_autocast():
     (loss_b, grads_b), rows = profiled(batch)
     assert rows and all(int(r["planes"]) == 0 for r in rows)
     loss_e, grads_e = explicit()
-    assert abs(loss_b - loss_e) <= RUN_OUT * abs(loss_e)
+    assert abs(loss_b - loss_e) <= parity.RUN_OUT * abs(loss_e)
     names = [k for k, _ in pipe.get_model().vision_model.named_parameters()]
-    close_grads(dict(zip(names, grads_b)), dict(zip(names, grads_e)))
+    parity.assert_same_run([], [], dict(zip(names, grads_b)), dict(zip(names, grads_e)))

@@ -16,18 +16,16 @@ sys.path.insert(0, os.path.join(HERE, "..", "ml-mdm_b200"))
 
 import fullwidth_cases as fc  # noqa: E402
 import lm_head_oracle  # noqa: E402
-import net_cases as nc  # noqa: E402
+import parity  # noqa: E402
 import tiny_configs as tc  # noqa: E402
 from mdm_b200 import _lib  # noqa: E402
 from mdm_b200 import config as mc  # noqa: E402
 from mdm_b200.diffusion import NestedDiffusion, NestedModel  # noqa: E402
-from mdm_b200.models import NestedUNet, UNet  # noqa: E402
+from mdm_b200.models import NestedUNet  # noqa: E402
 from mdm_b200.samplers import NestedSampler  # noqa: E402
 from oracle import unet_ref  # noqa: E402
 
 pytestmark = pytest.mark.gpu
-
-RUN_OUT, RUN_GRAD = 3e-3, 2e-2  # two engine runs (fp32 atomics add in a varying order)
 
 
 def build(kind, masked=1, layers=0, seed=7, dropout=0.0):
@@ -39,28 +37,12 @@ def build(kind, masked=1, layers=0, seed=7, dropout=0.0):
     while c is not None:
         c["resnet_config"]["dropout"] = dropout
         c = c.get("inner_config")
-    cfg = mc.unet_config_from_dict(ucfg)
-    cfg.conditioning_feature_dim = tc.LM_DIM
-    ocfg = copy.deepcopy(cfg)  # the model constructor mutates conditioning_feature_dim
-    model = (UNet if kind == "unet" else NestedUNet)(3, 3, cfg)
-    sd = tc.seeded_state_dict(model.state_dict(), seed)
-    model.load_state_dict(sd)
-    return model, lm_head_oracle.OracleNet(ocfg, tc.LM_DIM), sd
+    return parity.tiny_model(ucfg, lm_head_oracle.OracleNet, seed)
 
 
 def inputs(kind, seed=3, batch=2, tokens=6):
     nested = kind != "unet"
     return tc.seeded_inputs(seed, batch, 32 if nested else 16, tokens, nlevels=2 if nested else 1)
-
-
-class tf32:
-    def __enter__(self):
-        torch.backends.cuda.matmul.allow_tf32 = True
-        torch.backends.cudnn.allow_tf32 = True
-
-    def __exit__(self, *a):
-        torch.backends.cuda.matmul.allow_tf32 = False
-        torch.backends.cudnn.allow_tf32 = False
 
 
 def text_param(name):
@@ -81,14 +63,14 @@ def test_forward_conditioning_vs_oracle(kind, masked, layers):
         return lm_head_oracle.forward_conditioning(P, ipre, iplan, lm.to(dev, dt), mask.to(dev, dt))
 
     ref = ora("cpu", torch.float64)
-    with tf32():
+    with parity.tf32():
         t32 = ora("cuda", torch.float32)
     model = model.cuda()
     with torch.no_grad():
         emb, cond, cm = model.forward_conditioning(lm.cuda(), mask.cuda())
     assert (cm is None) == (masked == 0)
     for ours, r, t in ((emb, ref[0], t32[0]), (cond, ref[1], t32[1])):
-        e, et = nc.rel(ours.cpu().double(), r), nc.rel(t.cpu().double(), r)
+        e, et = parity.rel(ours.cpu(), r), parity.rel(t.cpu(), r)
         assert e <= max(2e-3, 2.0 * et), (e, et)
 
 
@@ -104,25 +86,18 @@ def test_forward_conditioning_fused_lm_mask():
     model.fuse_lm_mask = True
     with torch.no_grad():
         emb, cond, _ = model.forward_conditioning(raw.cuda(), mask.cuda())
-    assert nc.rel(cond.cpu().double(), ref[1]) <= 2e-3
-    assert nc.rel(emb.cpu().double(), ref[0]) <= 2e-3
+    assert parity.rel(cond.cpu(), ref[1]) <= 2e-3
+    assert parity.rel(emb.cpu(), ref[0]) <= 2e-3
 
 
 # ---------------------------------------------------------------- 2. forward_denoising on arbitrary inputs
-def _oracle_denoise(oracle, P, xs, t, cemb, cond, cmask):
-    ipre, iplan, _ = oracle.levels[-1]
-    if not oracle.nested:
-        return [unet_ref.unet_denoise(P, "", iplan, xs[0], t, cemb, cond, cmask, {})]
-    return list(oracle._nested(0, P, xs, None, t, cemb, cond, cmask, {}, None))
-
-
 @pytest.mark.parametrize("masked", [0, 1], ids=["m0", "m1"])
 @pytest.mark.parametrize("kind", ["unet", "nested"])
 def test_forward_denoising_random_inputs_vs_oracle(kind, masked):
     model, oracle, sd = build(kind, masked)
     x, t, _, _ = inputs(kind)
     xs = [x] if kind == "unet" else list(x)
-    ipre = oracle.levels[-1][0]
+    ipre, iplan, _ = oracle.levels[-1]
     td, cd = sd[ipre + "cond_emb.weight"].shape
     g = torch.Generator().manual_seed(17)
     B, S = xs[0].shape[0], 5
@@ -131,43 +106,27 @@ def test_forward_denoising_random_inputs_vs_oracle(kind, masked):
     cmask = torch.ones(B, S)
     cmask[1, 3:] = 0
     ws = [torch.randn(xi.shape, generator=g) for xi in xs]
+    # the conditioning tokens and embedding are leaves whose gradients are compared too; the tokens also fill the
+    # arms' text argument, which forward_denoising does not read
+    leaves = {"conditioning": cond, "cond_emb": cemb}
 
-    def ora(dev, dt):
-        P = {k: v.to(dev, dt).requires_grad_(True) for k, v in sd.items()}
-        c, e = cond.to(dev, dt).requires_grad_(True), cemb.to(dev, dt).requires_grad_(True)
-        outs = _oracle_denoise(oracle, P, [xi.to(dev, dt) for xi in xs], t.to(dev), e, c, cmask.to(dev, dt))
-        sum((o * w.to(dev, dt)).sum() for o, w in zip(outs, ws)).backward()
-        grads = {k: v.grad for k, v in P.items() if v.grad is not None}
-        grads["<conditioning>"], grads["<cond_emb>"] = c.grad, e.grad
-        return [o.detach().cpu().double() for o in outs], {k: v.cpu().double() for k, v in grads.items()}
+    def ora(P, x, t, lm, mask, micros, conditioning, cond_emb):
+        if not oracle.nested:
+            return unet_ref.unet_denoise(P, "", iplan, x, t, cond_emb, conditioning, mask, {})
+        return oracle._nested(0, P, x, None, t, cond_emb, conditioning, mask, {}, None)
 
-    r_out, r_g = ora("cpu", torch.float64)
-    with tf32():
-        t_out, t_g = ora("cuda", torch.float32)
-    model = model.cuda()
-    c = cond.cuda().requires_grad_(True)
-    e = cemb.cuda().requires_grad_(True)
-    xc = [xi.cuda() for xi in xs]
-    out = model.forward_denoising(xc[0] if kind == "unet" else xc, t.cuda(), e, c, cmask.cuda())
-    outs = [out] if kind == "unet" else out
-    sum((o * w.cuda()).sum() for o, w in zip(outs, ws)).backward()
-    for o, r, tt in zip(outs, r_out, t_out):
-        assert nc.rel(o.detach().cpu().double(), r) <= max(1e-3, 1.75 * nc.rel(tt, r))
-    ours = {k: p.grad for k, p in model.named_parameters() if p.grad is not None}
-    assert all(text_param(k) for k, p in model.named_parameters() if p.grad is None)
-    ours["<conditioning>"], ours["<cond_emb>"] = c.grad, e.grad
-    mags = sorted(float(r_g[k].abs().max()) for k in ours)
-    floor = 1e-2 * mags[len(mags) // 2]
-    err = {k: float((v.cpu().double() - r_g[k]).abs().max()) / max(float(r_g[k].abs().max()), floor) for k, v in ours.items()}
-    terr = {k: float((t_g[k] - r_g[k]).abs().max()) / max(float(r_g[k].abs().max()), floor) for k in ours}
-    med = sorted(terr.values())[len(terr) // 2]
-    bad = {k: (v, terr[k]) for k, v in err.items() if not v <= 3.5 * max(terr[k], med)}
-    assert not bad, bad
+    args = (sd, xs, t, cond, cmask, {}, ws)
+    f64 = parity.oracle_arm(ora, *args, torch.float64, "cpu", leaves=leaves)
+    t32 = parity.oracle_arm(ora, *args, torch.float32, "cuda", tf32=True, leaves=leaves)
+    ours = parity.engine_arm(model, xs, t, cond, cmask, {}, ws, leaves=leaves, forward=lambda x, t, lm, mask, micros,
+                             conditioning, cond_emb: model.forward_denoising(x, t, cond_emb, conditioning, mask))
+    assert all(text_param(k) for k, _ in model.named_parameters() if k not in ours[1])
+    parity.assert_calibrated(parity.report(ours, f64, t32))
 
 
 # ---------------------------------------------------------------- 3. split path against forward
 def _grads(m):
-    return {k: (p.grad.detach().clone() if p.grad is not None else None) for k, p in m.named_parameters()}
+    return {k: p.grad.detach().clone() for k, p in m.named_parameters() if p.grad is not None}
 
 
 @pytest.mark.parametrize("case", ["unet_l2", "nested", "nested_dropout", "nested_frozen_inner"])
@@ -195,24 +154,15 @@ def test_split_matches_forward(case):
     la.backward()
     lb.backward()
     torch.cuda.synchronize()
-    for u, v in zip(oa, ob):
-        assert nc.rel(v.detach(), u.detach()) <= RUN_OUT
     # the loss on the scale of its terms (it is a sum of terms of both signs)
     scale = float(sum((o.detach() * w).abs().sum() for o, w in zip(oa, ws)))
-    assert abs(float(la.detach()) - float(lb.detach())) <= RUN_OUT * scale
+    assert abs(float(la.detach()) - float(lb.detach())) <= parity.RUN_OUT * scale
     ga, gb = _grads(a), _grads(b)
-    mags = sorted(float(v.abs().max()) for v in ga.values() if v is not None)
-    floor = 1e-2 * mags[len(mags) // 2]
-    for k in ga:
-        assert (ga[k] is None) == (gb[k] is None), k
-        if ga[k] is None:
-            continue
-        e = float((gb[k] - ga[k]).abs().max()) / max(float(ga[k].abs().max()), floor)
-        assert e <= RUN_GRAD, (k, e)
+    parity.assert_same_run([v.detach() for v in ob], [u.detach() for u in oa], gb, ga)
     if "frozen" in case:
-        assert all(gb[k] is None for k in gb if k.startswith("inner_unet."))
+        assert not any(k.startswith("inner_unet.") for k in gb)
     else:
-        assert any(gb[k] is not None and text_param(k) for k in gb)
+        assert any(text_param(k) for k in gb)
 
 
 # ---------------------------------------------------------------- 4. the K/V cache
@@ -256,8 +206,8 @@ def test_cache_reads_back_what_a_fresh_fill_computes():
         ref = model(xs, t.cuda(), lm.cuda(), mask.cuda(), {})
     assert modes == [1, 2, 1]
     assert torch.equal(k1, k2) and torch.equal(k1, k3)
-    for a, b, r in zip(o1, o2, ref):
-        assert nc.rel(a, r) <= RUN_OUT and nc.rel(b, r) <= RUN_OUT
+    parity.assert_same_run(o1, ref)
+    parity.assert_same_run(o2, ref)
 
 
 def test_cache_invalidation():
@@ -275,11 +225,11 @@ def test_cache_invalidation():
         w.mul_(1.5)                                                     # in-place weight update
         o = model.forward_denoising(x, t, emb, cond, cm)
         ref = model.forward_denoising(x, t, emb, cond.clone(), cm)      # a different tensor
-        assert nc.rel(o, ref) <= RUN_OUT
+        parity.assert_same_run([o], [ref])
         cond.mul_(0.5)                                                  # in-place write to the tokens
         o = model.forward_denoising(x, t, emb, cond, cm)
         ref = model.forward_denoising(x, t, emb, cond.clone(), cm)
-        assert nc.rel(o, ref) <= RUN_OUT
+        parity.assert_same_run([o], [ref])
         model.forward_denoising(x, t, emb, cond, cm)
     assert modes == [1, 2, 1, 1, 1, 1, 1]
     # the engine itself refuses a stale or mismatched cache, whatever the caller asks for
@@ -320,13 +270,7 @@ def test_graph_replay_of_stage2_matches_eager():
                 inf = m.forward_denoising(xs, t.cuda(), emb, cond, cm)
             res.append(([o.detach() for o in outs], gr, inf))
         (og, gg, ig), (oe, ge, ie) = res
-        for a, b in zip(og + ig, oe + ie):
-            assert nc.rel(a, b) <= RUN_OUT, step
-        mags = sorted(float(v.abs().max()) for v in ge.values() if v is not None)
-        floor = 1e-2 * mags[len(mags) // 2]
-        for k in ge:
-            if ge[k] is not None:
-                assert float((gg[k] - ge[k]).abs().max()) / max(float(ge[k].abs().max()), floor) <= RUN_GRAD, (step, k)
+        parity.assert_same_run(og + ig, oe + ie, gg, ge)
     assert _lib.graph_launch_count() - g0 >= 4
 
 
@@ -358,18 +302,13 @@ def test_ddim_with_reuse_matches_per_step_forward_tiny_nest(guidance):
     # guidance amplifies the run-to-run differences of each evaluation (fp32 atomics) by 2w - 1 per step: the bound
     # is the spread of two runs of the per-step loop itself
     b2 = _sample(sampler, model, x, lm.cuda(), mask.cuda(), guidance, 8, True)
-    assert nc.rel(a, b) <= max(RUN_OUT, 3.0 * nc.rel(b2, b)), (nc.rel(a, b), nc.rel(b2, b))
+    assert parity.rel(a, b) <= max(parity.RUN_OUT, 3.0 * parity.rel(b2, b)), (parity.rel(a, b), parity.rel(b2, b))
 
 
 @pytest.mark.parametrize("guidance", [1.0, 3.0])
 def test_ddim_with_reuse_matches_per_step_forward_cc12m_256(guidance):
-    ucfg, dcfg, _ = mc.load_yaml_configs(os.path.join(fc.CFG_DIR, "cc12m_256x256.yaml"))
-    torch.manual_seed(4321)
-    vm = NestedUNet(3, 3, ucfg)
-    with torch.no_grad():
-        for p in vm.parameters():
-            if float(p.abs().max()) == 0:
-                p.normal_(0, 0.02)
+    _, dcfg, _ = mc.load_yaml_configs(os.path.join(fc.CFG_DIR, "cc12m_256x256.yaml"))
+    vm, _ = fc.build("cc12m_256x256", seed=4321)
     pipe = NestedDiffusion(vm, dcfg).to("cuda")
     pipe.eval()
     B = 2
@@ -382,7 +321,7 @@ def test_ddim_with_reuse_matches_per_step_forward_cc12m_256(guidance):
     x = torch.randn(B, 3, 256, 256, generator=g).cuda()
     a = _sample(pipe.sampler, pipe.get_model(), x, lm, mask * 1, guidance, 6, False)
     b = _sample(pipe.sampler, pipe.get_model(), x, lm, mask * 1, guidance, 6, True)
-    assert nc.rel(a, b) <= RUN_OUT
+    parity.assert_same_run([a], [b])
 
 
 def test_launches_drop_by_the_skipped_text_path():

@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 import torch
 
-import net_cases as nc
+import parity
 import tiny_configs as tc
 from mdm_b200 import config as mc
 from mdm_b200.diffusion import Diffusion, NestedDiffusion
@@ -18,7 +18,7 @@ GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 def pipeline(kind):
-    model, oracle, sd = nc.build(kind)
+    model, oracle, sd = parity.tiny_model(tc.TINY[kind])
     nested = kind == "nested"
     dcfg = mc.diffusion_config_from_dict(copy.deepcopy(tc.TINY_NESTED_DIFFUSION if nested else tc.TINY_DIFFUSION), nested)
     pipe = (NestedDiffusion if nested else Diffusion)(model, dcfg).to("cuda")
@@ -30,9 +30,7 @@ def pipeline(kind):
 def _calibrated_loss_check(pipe, oracle, sd, loss, P64, oloss, images, eps, time, lm, mask, scales, shifted, mixed_ratio=None):
     """loss and every parameter gradient of get_loss against the fp64 oracle, bounded by what the reference's own GPU
     arithmetic (the oracle in fp32 with TF32 on, same draws) scores on the same metric in the same run."""
-    torch.backends.cuda.matmul.allow_tf32 = True
-    torch.backends.cudnn.allow_tf32 = True
-    try:
+    with parity.tf32():
         P32 = {k: v.float().cuda().requires_grad_(True) for k, v in sd.items()}
         gam = dref.gammas_f32("DEEPFLOYD", 1000).cuda()
         tl, _, _ = dref.training_loss(oracle, P32, images.float().cuda(), [e.float().cuda() for e in eps], time.cuda(),
@@ -40,27 +38,14 @@ def _calibrated_loss_check(pipe, oracle, sd, loss, P64, oloss, images, eps, time
                                       shifted=shifted, power=1, mixed_ratio=mixed_ratio)
         tl.mean().backward()
         torch.cuda.synchronize()
-    finally:
-        torch.backends.cuda.matmul.allow_tf32 = False
-        torch.backends.cudnn.allow_tf32 = False
     ref_loss = oloss.detach()
-    e_ours = nc.rel(loss.detach().cpu().double(), ref_loss)
-    e_tf32 = nc.rel(tl.detach().cpu().double(), ref_loss)
+    e_ours = parity.rel(loss.detach().cpu(), ref_loss)
+    e_tf32 = parity.rel(tl.detach().cpu(), ref_loss)
     assert e_ours <= max(2e-3, 2.5 * e_tf32), (e_ours, e_tf32)  # per-sample loss: a mean over CHW of squared errors
-    mags = sorted(float(P64[k].grad.abs().max()) for k in P64)
-    floor = 1e-2 * mags[len(mags) // 2]
-    ours, tf32 = {}, {}
-    for k, p in pipe.get_model().vision_model.named_parameters():
-        ref = P64[k].grad
-        den = max(float(ref.abs().max()), floor)
-        ours[k] = float((p.grad.cpu().double() - ref).abs().max() / den)
-        tf32[k] = float((P32[k].grad.cpu().double() - ref).abs().max() / den)
-    t = sorted(tf32.values())
-    o = sorted(ours.values())
-    med = t[len(t) // 2]
-    assert o[len(o) // 2] <= 1.5 * med, (o[len(o) // 2], med)
-    bad = {k: (v, tf32[k]) for k, v in ours.items() if not (v <= 3.5 * max(tf32[k], med))}
-    assert not bad, bad
+    g64 = {k: v.grad for k, v in P64.items()}
+    ours = parity.grad_errors({k: p.grad.cpu() for k, p in pipe.get_model().vision_model.named_parameters()}, g64)
+    tf32 = parity.grad_errors({k: v.grad.cpu() for k, v in P32.items()}, g64)
+    parity.assert_calibrated_grads({k: (v, tf32[k]) for k, v in ours.items()})
 
 
 def test_q_sample_matches_to_one_ulp():
@@ -98,7 +83,7 @@ def test_get_loss_and_gradients(kind):
     gam = dref.gammas_f32("DEEPFLOYD", 1000)
     oloss, ox_t, _ = dref.training_loss(oracle, P, images.double(), [e.cpu().double() for e in eps], time.cpu(), lm.double(), mask.double(),
                                         gam, scales, dref.V_PREDICTION, dref.DDPM, shifted=nested, power=1)
-    assert nc.rel(x_t.cpu().double(), ox_t[0]) <= 1e-6
+    assert parity.rel(x_t.cpu().double(), ox_t[0]) <= 1e-6
     oloss.mean().backward()
     _calibrated_loss_check(pipe, oracle, sd, loss, P, oloss, images, [e.cpu() for e in eps], time.cpu(), lm, mask, scales,
                            shifted=nested)
@@ -120,13 +105,13 @@ def test_reverse_steps_vs_reference_golden(kind):
         for i, (a, b) in enumerate(zip(x0, xs) if nested else [(x0, xs)]):
             # one network evaluation (<= 2e-3 on v) pushed through x0 = a x_t - c v and the clip
             # (single-evaluation bound 2.5e-3, amplified by 1/sqrt(gamma) ~ 1.4-2 in x0 = a x_t - c v)
-            assert nc.rel(a.cpu(), torch.from_numpy(gold[f"ddim_x0_{i}"])) <= 5e-3
-            assert nc.rel(b.cpu(), torch.from_numpy(gold[f"ddim_xs_{i}"])) <= 5e-3
+            assert parity.rel(a.cpu(), torch.from_numpy(gold[f"ddim_x0_{i}"])) <= 5e-3
+            assert parity.rel(b.cpu(), torch.from_numpy(gold[f"ddim_xs_{i}"])) <= 5e-3
         lm2 = torch.cat([torch.zeros_like(lmc), lmc])
         xs = smp.get_xt_minus_1(m, 500, clone(xc), lm2, torch.cat([mc_, mc_]), {}, time_step_last=480, ddim_eta=0.0,
                                 guidance_scale=3.0)
         for i, b in enumerate(xs if nested else [xs]):
-            assert nc.rel(b.cpu(), torch.from_numpy(gold[f"cfg_xs_{i}"])) <= 5e-3
+            assert parity.rel(b.cpu(), torch.from_numpy(gold[f"cfg_xs_{i}"])) <= 5e-3
         # stochastic DDPM step: noise comes from the CUDA generator, so compare against the oracle's
         # deterministic part (posterior mean) by replaying the same noise
         torch.manual_seed(99)
@@ -142,7 +127,7 @@ def test_reverse_steps_vs_reference_golden(kind):
         for xi, p, s, nz, got in zip(x if nested else [x], preds, scales, noises, lv):
             tab = dref.shift_table(gam, s, 1) if nested else gam
             _, ref = dref.reverse_step(xi, p.cpu(), tab[500], tab[499], dref.V_PREDICTION, True, 1.0, None, True, noise=nz.cpu())
-            assert nc.rel(got.cpu(), ref) <= 1e-5
+            assert parity.rel(got.cpu(), ref) <= 1e-5
 
 
 @pytest.mark.parametrize("kind", ["unet", "nested"])
@@ -158,7 +143,7 @@ def test_ddim_sampling_vs_reference_golden(kind):
         init = x.cuda()
     out = smp.sample(m, init, lm.cuda(), mask.cuda(), {}, num_inference_steps=4, ddim_eta=0.0, resample_steps=True)
     # four chained network evaluations, each within the single-evaluation bound of tests/test_net_gpu.py (2.5e-3)
-    assert nc.rel(out.cpu(), torch.from_numpy(gold["sample4"])) <= 4 * 2.5e-3
+    assert parity.rel(out.cpu(), torch.from_numpy(gold["sample4"])) <= 4 * 2.5e-3
     assert float(out.abs().max()) <= 1.0
 
 
@@ -180,7 +165,7 @@ def test_get_loss_mixed_ratio_batches():
     the loss is rescaled and masked. Oracle: oracle.diffusion_ref.training_loss(mixed_ratio=...) -- itself pinned
     against the live reference in tests/test_oracle.py."""
     B = 3
-    model, oracle, sd = nc.build("nested")
+    model, oracle, sd = parity.tiny_model(tc.TINY_NESTED)
     d = copy.deepcopy(tc.TINY_NESTED_DIFFUSION)
     d["mixed_ratio"] = "2:1"
     pipe = NestedDiffusion(model, mc.diffusion_config_from_dict(d, True)).to("cuda")
@@ -253,13 +238,13 @@ def test_dynamic_threshold_reverse_step_and_sampling(mode):
             tab = dref.shift_table(gam, s, 1)
             r0, rs = dref.reverse_step(xi.cpu(), p.cpu(), tab[500], tab[480], dref.V_PREDICTION, mode, 1.0, 0.0, True)
             assert float(r0.abs().max()) <= 1.0 + 1e-6
-            assert nc.rel(a.cpu(), r0) <= 2e-6 and nc.rel(b.cpu(), rs) <= 2e-6
+            assert parity.rel(a.cpu(), r0) <= 2e-6 and parity.rel(b.cpu(), rs) <= 2e-6
         x0, xs, _ = smp.get_xt_minus_1(m, 500, [a.clone() for a in xc], lmc, mc_, {}, time_step_last=480, ddim_eta=0.0,
                                        return_details=True)
         assert all(float(a.abs().max()) <= 1.0 + 1e-6 for a in x0)
     # clip_sample on a bare tensor (reference surface)
     t = (torch.randn(2, 3, 16, 16) * 2).cuda()
-    assert nc.rel(smp.clip_sample(t, 2.0).cpu(), dref.clip_sample(t.cpu(), 2.0, mode)) <= 1e-6
+    assert parity.rel(smp.clip_sample(t, 2.0).cpu(), dref.clip_sample(t.cpu(), 2.0, mode)) <= 1e-6
     torch.manual_seed(0)
     out = pipe.sample(2, {"lm_outputs": lmc, "lm_mask": mc_}, 32, torch.device("cuda"), num_inference_steps=3,
                       ddim_eta=0.0, resample_steps=True)
@@ -296,9 +281,5 @@ def test_get_loss_from_raw_reader_batch_uint8_and_unmasked_t5(kind):
     lb, tb, xb, tgb, gb = run({"image": u8, "lm_outputs": lm_raw, "lm_mask": mask, "lm_mask_applied": False})
     assert torch.equal(ta, tb)
     assert torch.equal(xa, xb) and torch.equal(tga, tgb), "fused uint8 q-sample must be bit-identical"
-    assert nc.rel(lb, la) <= 3e-3           # two engine runs differ by fp32-atomic order only
-    mags = sorted(float(v.abs().max()) for v in ga.values())
-    floor = 1e-2 * mags[len(mags) // 2]
-    for k in ga:
-        assert float((gb[k] - ga[k]).abs().max()) <= 2e-2 * max(float(ga[k].abs().max()), floor), k  # run-to-run level
+    parity.assert_same_run([lb], [la], gb, ga)  # two engine runs differ by fp32-atomic order only
     assert vm.fuse_lm_mask is False

@@ -1,7 +1,6 @@
 """ResNet dropout (ResNetConfig.dropout) on the GPU: the mask operator's statistics, and the native UNet / NestedUNet in
 train mode against the dropout oracle fed with the engine's own masks (rebuilt by mdm_op_dropout_mask from the seed the
 model draws from torch's CPU generator), eval mode, no_grad, p = 1, CUDA-graph replay and a full-width nested step."""
-import copy
 import ctypes as C
 import os
 import sys
@@ -14,12 +13,12 @@ sys.path.insert(0, HERE)
 sys.path.insert(0, os.path.join(HERE, "..", "ml-mdm_b200"))
 
 import dropout_oracle  # noqa: E402
+import fullwidth_cases as fc  # noqa: E402
 import net_cases as nc  # noqa: E402
+import parity  # noqa: E402
 import test_dropout_host as host  # noqa: E402
 import tiny_configs as tc  # noqa: E402
 from mdm_b200 import _lib  # noqa: E402
-from mdm_b200 import config as mc  # noqa: E402
-from mdm_b200.models import NestedUNet, UNet  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -76,48 +75,34 @@ def test_mask_operator_statistics(p):
 
 
 # ------------------------------------------------------------------------------------------ the network
-def tiny_build(masked, p_outer=host.P_OUTER, p_inner=host.P_INNER):
-    """net_cases.build for the tiny configs with dropout, whose oracle applies the engine's masks of the forward that
-    follows (run_case runs the native model once, right after build)."""
-    def build(kind, seed=7):
-        ucfg = host.tiny_config("unet" if kind == "unet" else "nested_unet", p_outer, p_inner)
-        (ucfg if kind == "unet" else ucfg["inner_config"])["masked_cross_attention"] = masked
-        cfg = mc.unet_config_from_dict(ucfg)
-        cfg.conditioning_feature_dim = tc.LM_DIM
-        ocfg = copy.deepcopy(cfg)
-        model = (UNet if kind == "unet" else NestedUNet)(3, 3, cfg)
-        sd = tc.seeded_state_dict(model.state_dict(), seed)
-        model.load_state_dict(sd)
-        oracle = dropout_oracle.OracleNet(ocfg, tc.LM_DIM, mask_fn(model, seed_after(DROP_SEED), [p_outer, p_inner]))
-        torch.manual_seed(DROP_SEED)
-        return model, oracle, sd
-    return build
+def tiny_build(kind, masked, p_outer=host.P_OUTER, p_inner=host.P_INNER, seed=7):
+    """parity.tiny_model of the tiny config with dropout, whose oracle applies the engine's masks of the next forward:
+    the torch seed is set to DROP_SEED on return."""
+    ucfg = host.tiny_config("unet" if kind == "unet" else "nested_unet", p_outer, p_inner)
+    (ucfg if kind == "unet" else ucfg["inner_config"])["masked_cross_attention"] = masked
+    model, oracle, sd = parity.tiny_model(ucfg, dropout_oracle.OracleNet, seed, masks=None)
+    oracle.masks = mask_fn(model, seed_after(DROP_SEED), [p_outer, p_inner])
+    torch.manual_seed(DROP_SEED)
+    return model, oracle, sd
 
 
 @pytest.mark.parametrize("masked", [0, 1], ids=["m0", "m1"])
 @pytest.mark.parametrize("kind", ["unet", "nested"])
-def test_dropout_forward_backward_vs_oracle(kind, masked, monkeypatch):
-    monkeypatch.setattr(nc, "build", tiny_build(masked))
-    nc.assert_calibrated(nc.run_case(kind, verbose=False))
+def test_dropout_forward_backward_vs_oracle(kind, masked):
+    parity.assert_calibrated(nc.run_case(kind, tiny_build(kind, masked), verbose=False))
 
 
-def test_dropout_mixed_ratio_nest_vs_oracle(monkeypatch):
+def test_dropout_mixed_ratio_nest_vs_oracle():
     """The outer level runs the first sample only (level_batch 1 of 2): its masks index a (1, H, W, C) tensor."""
-    monkeypatch.setattr(nc, "build", tiny_build(1))
-    real = tc.seeded_inputs
-
-    def narrow_outer(*a, **k):
-        xs, t, lm, mask = real(*a, **k)
-        return [xs[0][:1]] + xs[1:], t, lm, mask
-
-    monkeypatch.setattr(nc.tc, "seeded_inputs", narrow_outer)
-    nc.assert_calibrated(nc.run_case("nested", verbose=False))
+    xs, t, lm, mask = tc.seeded_inputs(3, 2, 32, 6, nlevels=2)
+    built = tiny_build("nested", 1)
+    parity.assert_calibrated(nc.run_case("nested", built, ([xs[0][:1]] + xs[1:], t, lm, mask), verbose=False))
 
 
 def test_dropout_p1_gives_reference_zeros():
     """p = 1: every ResNet's conv2 sees zeros (nn.Dropout(p=1)), so the gradients inside the ResNets are exactly zero,
     not NaN, and the rest of the step matches the oracle with all-zero masks."""
-    model, oracle, sd = tiny_build(1, 1.0, 1.0)("nested")
+    model, oracle, sd = tiny_build("nested", 1, 1.0, 1.0)
     x, t, lm, mask = _inputs("nested")
     P = {k: v.double().requires_grad_(True) for k, v in sd.items()}
     ref = oracle.forward(P, [xi.cpu().double() for xi in x], t.cpu(), lm.cpu().double(), mask.cpu().double(), {})
@@ -126,9 +111,8 @@ def test_dropout_p1_gives_reference_zeros():
     out = model(x, t, lm, mask, {})
     sum((o * o).sum() for o in out).backward()
     for o, r in zip(out, ref):
-        assert nc.rel(o.detach().cpu().double(), r.detach()) <= 2.5e-3
-    mags = sorted(float(P[k].grad.abs().max()) for k in P if float(P[k].grad.abs().max()) > 0)
-    floor = 1e-2 * mags[len(mags) // 2]
+        assert parity.rel(o.detach().cpu(), r.detach()) <= 2.5e-3
+    floor = parity.grad_floor({k: v.grad for k, v in P.items() if float(v.grad.abs().max()) > 0})
     inside = (".norm1.", ".conv1.", ".time_layer.", ".norm2.", ".conv2.weight")
     for k, p in model.named_parameters():
         g = p.grad.detach().cpu().double()
@@ -141,8 +125,8 @@ def test_dropout_p1_gives_reference_zeros():
             assert float((g - P[k].grad).abs().max()) / float(P[k].grad.abs().max()) <= 5e-2, k
 
 
-def _model(kind, p_outer, p_inner, seed=7):
-    return tiny_build(1, p_outer, p_inner)(kind, seed)[0].cuda()
+def _model(kind, p_outer, p_inner):
+    return tiny_build(kind, 1, p_outer, p_inner)[0].cuda()
 
 
 def _inputs(kind, seed=3):
@@ -163,8 +147,7 @@ def test_eval_mode_runs_as_p0(kind):
     a, b = _model(kind, 0.1, 0.25).eval(), _model(kind, 0.0, 0.0).eval()
     inp = _inputs(kind)
     with torch.no_grad():
-        for x, y in zip(_outs(a(*inp, {})), _outs(b(*inp, {}))):
-            assert nc.rel(x, y) <= 3e-3, nc.rel(x, y)
+        parity.assert_same_run(_outs(a(*inp, {})), _outs(b(*inp, {})))
 
 
 @pytest.mark.parametrize("kind", ["unet", "nested"])
@@ -174,7 +157,7 @@ def test_no_grad_forward_in_train_mode_drops(kind):
     with torch.no_grad():
         train = _outs(m(*inp, {}))
         ev = _outs(m.eval()(*inp, {}))
-    assert all(nc.rel(x, y) > 1e-2 for x, y in zip(train, ev)), [nc.rel(x, y) for x, y in zip(train, ev)]
+    assert all(parity.rel(x, y) > 1e-2 for x, y in zip(train, ev)), [parity.rel(x, y) for x, y in zip(train, ev)]
 
 
 def test_nested_dropout_modules_disagreeing_with_the_model_are_refused():
@@ -222,43 +205,21 @@ def test_graph_steps_match_eager_steps_under_one_seed(kind):
     assert _lib.graph_launch_count() - g0 >= 4  # steps 2-4 replayed forward and backward graphs
     torch.manual_seed(77)
     esteps = [_step(eager, inp) for _ in range(4)]
-    for i, ((og, gg), (oe, ge)) in enumerate(zip(gsteps, esteps)):
-        for a, b in zip(og, oe):
-            assert nc.rel(a, b) <= 3e-3, (i, nc.rel(a, b))
-        mags = sorted(float(v.abs().max()) for v in ge.values())
-        floor = 1e-2 * mags[len(mags) // 2]
-        for k in ge:
-            e = float((gg[k] - ge[k]).abs().max() / max(float(ge[k].abs().max()), floor))
-            assert e <= 2e-2, (i, k, e)
+    for (og, gg), (oe, ge) in zip(gsteps, esteps):
+        parity.assert_same_run(og, oe, gg, ge)
     # consecutive steps draw fresh masks, replays included: identical inputs, different outputs
     for i in range(1, 4):
-        assert all(nc.rel(a, b) > 1e-2 for a, b in zip(gsteps[i][0], gsteps[i - 1][0])), i
+        assert all(parity.rel(a, b) > 1e-2 for a, b in zip(gsteps[i][0], gsteps[i - 1][0])), i
 
 
-def test_full_width_nested_step_with_dropout(monkeypatch):
+def test_full_width_nested_step_with_dropout():
     """One cc12m_256x256 training step with p = 0.1 on both levels, bounds of test_fullwidth_gpu."""
-    import fullwidth_cases as fc
-    import test_fullwidth_gpu as tfw
-
-    real_build = fc.build
-    state = {}
-
-    def build(name, seed=0):
-        ucfg, _, nested = mc.load_yaml_configs(os.path.join(fc.CFG_DIR, name + ".yaml"))
-        c = ucfg
+    def dropout(c):
         while c is not None:
             c.resnet_config.dropout = 0.1
             c = getattr(c, "inner_config", None)
-        ocfg = copy.deepcopy(ucfg)
-        m, _, _ = real_build(name, seed)
-        dm = (NestedUNet if nested else UNet)(3, 3, ucfg)
-        dm.load_state_dict(m.state_dict())
-        state["masks"] = mask_fn(dm, seed_after(DROP_SEED), [0.1, 0.1])
-        torch.manual_seed(DROP_SEED)
-        return dm, ocfg, nested
 
-    oracle_mod = type(sys)("dropout_unet_ref")
-    oracle_mod.OracleNet = lambda cfg, lm_dim: dropout_oracle.OracleNet(cfg, lm_dim, state["masks"])
-    monkeypatch.setattr(fc, "build", build)
-    monkeypatch.setattr(fc, "unet_ref", oracle_mod)
-    tfw.test_forward_backward_full_width_calibrated_against_reference_tf32("cc12m_256x256", 2)
+    m, ocfg = fc.build("cc12m_256x256", edit=dropout)
+    oracle = dropout_oracle.OracleNet(ocfg, 2048, mask_fn(m, seed_after(DROP_SEED), [0.1, 0.1]))
+    torch.manual_seed(DROP_SEED)
+    parity.assert_calibrated_full_width(fc.run_case("cc12m_256x256", m, oracle, B=2, S=8, micro=True))

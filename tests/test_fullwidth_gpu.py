@@ -18,27 +18,13 @@ magnitude the reference-TF32 path leaves in the same tensor (or 1e-3 of the typi
 import pytest
 
 import fullwidth_cases as fc
+import parity
+from oracle import unet_ref
 
 pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("name,batch", [("cc12m_64x64", 2), ("cc12m_256x256", 2), ("cc12m_1024x1024", 1)])
 def test_forward_backward_full_width_calibrated_against_reference_tf32(name, batch):
-    rep = fc.run_case(name, B=batch, S=8, micro=True)
-    assert not rep["missing"], rep["missing"]
-    for i, (ours, tf32) in enumerate(rep["out"]):
-        assert ours <= max(1e-3, 1.5 * tf32), (name, i, ours, tf32)
-    defined = {k: v for k, v in rep["grads"].items() if v[1] <= 0.5}
-    undefined = {k: v for k, v in rep["grads"].items() if v[1] > 0.5}
-    assert len(undefined) <= 0.05 * len(rep["grads"]), sorted(undefined)[:10]
-    for k in undefined:  # zero by construction: round-off of the size the reference's own TF32 path leaves there
-        lim = 3.0 * max(rep["grad_absmax_tf32"][k], 1e-3 * rep["grad_typical"])
-        assert rep["grad_absmax"][k] <= lim, (k, rep["grad_absmax"][k], rep["grad_absmax_tf32"][k], rep["grad_typical"])
-    o = sorted(v[0] for v in defined.values())
-    r = sorted(v[1] for v in defined.values())
-    n = len(o)
-    assert o[n // 2] <= 1.25 * r[n // 2], (o[n // 2], r[n // 2])
-    assert o[int(0.9 * n)] <= 1.25 * r[int(0.9 * n)], (o[int(0.9 * n)], r[int(0.9 * n)])
-    med = r[n // 2]
-    bad = {k: v for k, v in defined.items() if v[0] > 3.0 * max(v[1], med)}
-    assert not bad, bad
+    m, ocfg = fc.build(name)
+    parity.assert_calibrated_full_width(fc.run_case(name, m, unet_ref.OracleNet(ocfg, 2048), B=batch, S=8, micro=True))

@@ -17,7 +17,7 @@ import torch.nn as nn
 
 import algebra_cases as ac
 import multistep_oracle as mo
-import net_cases as nc
+import parity
 import test_rect_oracle as fx
 import tiny_configs as tc
 from mdm_b200 import config as mc
@@ -262,7 +262,7 @@ TINY = [("unet", None, 1, "CLIP", "dpmpp_2m"), ("unet", (24, 40), 5, "DYNAMIC", 
 @pytest.mark.parametrize("kind,hw,gs,thr,solver", TINY, ids=lambda v: str(v))
 def test_tiny_nets(kind, hw, gs, thr, solver, steps, worst):
     nested = kind == "nested"
-    model = nc.build(kind)[0]
+    model = parity.tiny_model(tc.TINY[kind])[0]
     dcfg = copy.deepcopy(tc.TINY_NESTED_DIFFUSION if nested else tc.TINY_DIFFUSION)
     dcfg["sampler_config"]["threshold_function"] = thr
     pipe = (NestedDiffusion if nested else Diffusion)(model, mc.diffusion_config_from_dict(dcfg, nested)).to("cuda")

@@ -13,7 +13,10 @@ import numpy as np
 import pytest
 import torch
 
+import fullwidth_cases as fc
 import net_cases as nc
+import parity
+import tiny_configs as tc
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -21,16 +24,13 @@ GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 @pytest.mark.parametrize("kind", ["unet", "nested"])
 def test_forward_backward_vs_oracle(kind):
-    r = nc.run_case(kind, verbose=False)
-    nc.assert_calibrated(r)
+    parity.assert_calibrated(nc.run_case(kind, verbose=False))
 
 
 @pytest.mark.parametrize("kind", ["unet", "nested"])
 def test_forward_vs_reference_golden(kind):
     """Same inputs/parameters as tests/golden (generated from the unmodified reference in fp32)."""
-    import tiny_configs as tc
-
-    model, _, _ = nc.build(kind)
+    model, _, _ = parity.tiny_model(tc.TINY[kind])
     nested = kind == "nested"
     x, t, lm, mask = tc.seeded_inputs(3, 2, 32 if nested else 16, 6, nlevels=2 if nested else 1)
     gold = np.load(os.path.join(GOLD, f"tiny_{kind}.npz"))
@@ -39,7 +39,7 @@ def test_forward_vs_reference_golden(kind):
         out = model([xi.cuda() for xi in x] if nested else x.cuda(), t.cuda(), lm.cuda(), mask.cuda(), {})
     for i, o in enumerate(out if nested else [out]):
         ref = torch.from_numpy(gold[f"fwd_out{i}"])
-        assert nc.rel(o.cpu(), ref) <= 2.5e-3  # ~1.75 x the reference-TF32 error of these outputs (1.0-1.3e-3)
+        assert parity.rel(o.cpu(), ref) <= 2.5e-3  # ~1.75 x the reference-TF32 error of these outputs (1.0-1.3e-3)
 
 
 def test_fresh_model_outputs_exact_zero():
@@ -60,17 +60,7 @@ def test_fresh_model_outputs_exact_zero():
 
 def test_batch_independence_full_width():
     """Every op is per-sample (no BatchNorm): sample i's output must not depend on its batch mates."""
-    from mdm_b200 import config as mc
-    from mdm_b200.models import UNet
-
-    cfgp = os.path.join(os.path.dirname(GOLD), "..", "ml-mdm_b200", "mdm_b200", "configs", "cc12m_64x64.yaml")
-    ucfg, _, _ = mc.load_yaml_configs(cfgp)
-    torch.manual_seed(0)
-    m = UNet(3, 3, ucfg)
-    with torch.no_grad():
-        for p in m.parameters():
-            if float(p.abs().max()) == 0:
-                p.normal_(0, 0.02)
+    m, _ = fc.build("cc12m_64x64")
     m = m.cuda()
     x = torch.randn(3, 3, 64, 64, device="cuda")
     t = torch.tensor([10, 500, 990], device="cuda")
@@ -81,8 +71,8 @@ def test_batch_independence_full_width():
         one = m(x[1:2], t[1:2], lm[1:2], mask[1:2], {})
     # Not bit-identical: the GroupNorm partial sums are combined by fp32 atomics whose order depends on
     # the grid, and a 1e-7 change upstream flips fp16 roundings (2^-11 each) downstream -- the same
-    # noise floor as the parity bound, far below any cross-sample leak (which would be O(1)).
-    assert nc.rel(one, full[1:2]) <= 3e-3
+    # noise floor as two runs of one batch, far below any cross-sample leak (which would be O(1)).
+    assert parity.rel(one, full[1:2]) <= parity.RUN_OUT
 
 
 # (full-width forward AND backward parity of the three shipped configs: tests/test_fullwidth_gpu.py)
@@ -95,10 +85,12 @@ def test_grad_ready_ranges_are_final(kind):
     already hold its final values in stream order (this is what lets the data-parallel all-reduce start
     before backward has finished, parallel.GradientOverlap). A snapshot enqueued inside the callback is
     compared bit-for-bit with the arena after backward."""
-    import tiny_configs as tc
+    check_grad_ready_ranges(parity.tiny_model(tc.TINY[kind])[0], kind)
+
+
+def check_grad_ready_ranges(model, kind):
     nlev = 1 if kind == "unet" else 2
     res = 16 if kind == "unet" else 32
-    model, _, _ = nc.build(kind)
     model = model.cuda()
     x, t, lm, mask = tc.seeded_inputs(3, 2, res, 6, nlevels=nlev)
     xs = [x.cuda()] if nlev == 1 else [xi.cuda() for xi in x]

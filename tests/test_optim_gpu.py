@@ -97,9 +97,9 @@ def test_fused_adam_on_tiny_unet_matches_separate_calls():
     """Two optimisation steps of a tiny U-Net: FusedAdam.step(clip, ema) on the engine's gradient arena vs
     clip_grad_norm_ + torch Adam + ModelEma.update on a copy that is handed the very same gradients (Adam divides
     by sqrt(v): feeding both sides one set of gradients keeps round-off-sized gradients from deciding signs)."""
-    import net_cases as nc
+    import parity
     import tiny_configs as tc
-    model_a, _, _ = nc.build("unet")
+    model_a, _, _ = parity.tiny_model(tc.TINY_UNET)
     model_a = model_a.cuda()
     model_b = copy.deepcopy(model_a)
     x, t, lm, mask = tc.seeded_inputs(3, 2, 16, 6, nlevels=1)
@@ -135,10 +135,10 @@ def test_fused_adam_on_tiny_unet_matches_separate_calls():
 
 
 def _tiny(kind="unet"):
-    import net_cases as nc
+    import parity
     import tiny_configs as tc
     nlev = 1 if kind == "unet" else 2
-    model, _, _ = nc.build(kind)
+    model, _, _ = parity.tiny_model(tc.TINY[kind])
     model = model.cuda()
     x, t, lm, mask = tc.seeded_inputs(3, 2, 16 if nlev == 1 else 32, 6, nlevels=nlev)
     xs = x.cuda() if nlev == 1 else [xi.cuda() for xi in x]

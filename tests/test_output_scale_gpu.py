@@ -11,7 +11,7 @@ import numpy as np
 import pytest
 import torch
 
-import net_cases as nc
+import parity
 import test_rect_oracle as fx
 from mdm_b200 import config as mc
 from mdm_b200.diffusion import Diffusion, Model, NestedModel
@@ -33,7 +33,7 @@ def _cfg(s, nested=False):
 
 @pytest.mark.parametrize("s", [0.1, 1.0, 4.0])
 def test_forward_is_tanh_of_the_unscaled_output(s):
-    vm, _, _ = nc.build("unet")
+    vm, _, _ = parity.tiny_model(fx.tc.TINY_UNET)
     vm = vm.cuda()
     inp = _unet_inputs()
     with torch.no_grad():
@@ -51,7 +51,7 @@ def test_forward_is_tanh_of_the_unscaled_output(s):
 # factor, so the gradients of two calls agree only to that
 @pytest.mark.parametrize("s,med_tol,max_tol", [(0.1, 1e-2, 5e-2), (1.0, 3e-3, 2e-2), (4.0, 3e-3, 2e-2)])
 def test_gradient_matches_autograd_through_tanh(s, med_tol, max_tol):
-    vm, _, _ = nc.build("unet")
+    vm, _, _ = parity.tiny_model(fx.tc.TINY_UNET)
     vm = vm.cuda()
     inp = _unet_inputs()
     g = torch.Generator().manual_seed(17)
@@ -68,9 +68,7 @@ def test_gradient_matches_autograd_through_tanh(s, med_tol, max_tol):
         vm.zero_grad(set_to_none=True)
     torch.cuda.synchronize()
     ref, got = grads
-    mags = sorted(float(v.abs().max()) for v in ref.values())
-    floor = 1e-2 * mags[len(mags) // 2]
-    errs = sorted(float((got[k] - v).abs().max()) / max(float(v.abs().max()), floor) for k, v in ref.items())
+    errs = sorted(parity.grad_errors(got, ref).values())
     assert errs[len(errs) // 2] <= med_tol and errs[-1] <= max_tol, (errs[len(errs) // 2], errs[-1])
 
 
@@ -79,7 +77,7 @@ def test_get_loss_matches_reference_fixture():
     then the per-sample loss of Diffusion.get_loss, against the reference's loss."""
     gold = np.load(fx.GOLD)
     tag, h, w, s = "u24x40_s", 24, 40, 0.1
-    vm, _, _ = nc.build("unet")
+    vm, _, _ = parity.tiny_model(fx.tc.TINY_UNET)
     model = Model(vm.cuda(), _cfg(s))
     x, _, lm, mask = fx.rect_inputs(3, 2, (h, w), 6)
     images = x.clamp(-1, 1)
@@ -101,7 +99,7 @@ def test_ddim50_cfg_encoded_once_matches_per_step():
         def forward(self, *a, **k):
             return super().forward(*a, **k)
 
-    vm, _, _ = nc.build("unet")
+    vm, _, _ = parity.tiny_model(fx.tc.TINY_UNET)
     vm = vm.cuda()
     pipe = Diffusion(vm, _cfg(0.1)).to("cuda")
     _, _, lm, mask = _unet_inputs()
@@ -114,8 +112,8 @@ def test_ddim50_cfg_encoded_once_matches_per_step():
         imgs.append(pipe.sampler.sample(m, noise, lm2, mask2, {}, num_inference_steps=50, resample_steps=True,
                                         ddim_eta=0.0, guidance_scale=3.0))
     torch.cuda.synchronize()
-    assert nc.rel(imgs[0], imgs[1]) <= max(3e-3, 3.0 * nc.rel(imgs[2], imgs[0])), (nc.rel(imgs[0], imgs[1]),
-                                                                                nc.rel(imgs[2], imgs[0]))
+    a, spread = parity.rel(imgs[0], imgs[1]), parity.rel(imgs[2], imgs[0])
+    assert a <= max(parity.RUN_OUT, 3.0 * spread), (a, spread)
 
 
 def _spy(native):
@@ -130,7 +128,7 @@ def _spy(native):
 
 
 def test_nested_model_and_direct_unet_are_never_scaled():
-    vm, _, _ = nc.build("nested")
+    vm, _, _ = parity.tiny_model(fx.tc.TINY_NESTED)
     vm = vm.cuda()
     xs, t, lm, mask = fx.rect_inputs(3, 2, fx.NEST_HW, 6, nlevels=2)
     inp = ([x.cuda() for x in xs], t.cuda(), lm.cuda(), mask.cuda())
@@ -140,10 +138,10 @@ def test_nested_model_and_direct_unet_are_never_scaled():
         b = vm(*inp, {})
     # the engine runs the same unscaled code path (the scale reaches it as 0) for both calls
     assert seen == [0.0, 0.0]
-    for p, q in zip(a, b):
-        assert nc.rel(p, q) <= 3e-3
+    parity.assert_same_run(a, b)
+    for p in a:
         assert float(p.abs().max()) > 0.15  # not squashed into (-0.1, 0.1)
-    u, _, _ = nc.build("unet")
+    u, _, _ = parity.tiny_model(fx.tc.TINY_UNET)
     u = u.cuda()
     seen = _spy(u.native())
     Model(u, _cfg(0.1))  # constructing the pipeline model changes nothing about direct calls
@@ -156,7 +154,7 @@ def test_nested_model_and_direct_unet_are_never_scaled():
 
 
 def test_graph_replay_follows_the_scale():
-    vm, _, _ = nc.build("unet")
+    vm, _, _ = parity.tiny_model(fx.tc.TINY_UNET)
     eager = copy.deepcopy(vm).cuda()
     graph = vm.cuda()
     eager.native().set_graph_mode(False)
@@ -173,6 +171,6 @@ def test_graph_replay_follows_the_scale():
         # absolute: with |y| <= s the relative metric inflates the unscaled outputs' ~1e-3 spread by 1/s, while a graph
         # replaying another s is off by up to |s - s'|
         assert float((outs[0][0] - outs[1][0]).abs().max()) <= 1e-2, (step, s)
-        assert nc.rel(outs[0][1], outs[1][1]) <= 5e-2, (step, s)
+        assert parity.rel(outs[0][1], outs[1][1]) <= 5e-2, (step, s)
         if s:
             assert float(outs[0][0].abs().max()) <= s * (1 + 1e-6)  # |s tanh| <= s, up to fp32 rounding of s

@@ -68,6 +68,7 @@ TINY_NESTED = dict(
 )
 # inner net must start at the outer net's last width for in/out adapters (any widths are legal)
 TINY_NESTED["inner_config"]["temporal_dim"] = None
+TINY = {"unet": TINY_UNET, "nested": TINY_NESTED}
 
 TINY_NESTED_DIFFUSION = dict(
     sampler_config=dict(num_diffusion_steps=1000, reproject_signal=False,
